@@ -4,14 +4,16 @@
 // activations, applied AdaIN / Snake / LeakyReLU and wrote them back to HBM as bf16 (hi, lo) planes, and the tensor-core GEMM that
 // read those planes once per tap.  This kernel does all of it in ONE launch and reads the activations ONCE:
 //
-//   converter warps (8)  fp32 activations (global, coalesced float4) -> [AdaIN scale/shift from the producer's (sum, sumsq)] ->
+//   worker warps (8)     (2 warpgroups; also run the epilogue below)
+//                        fp32 activations (global, coalesced float4) -> [AdaIN scale/shift from the producer's (sum, sumsq)] ->
 //                        Snake / LeakyReLU / ELU -> bf16 (or fp16) hi + lo planes written straight into the 128B-swizzled shared-memory
 //                        tile the MMA consumes.  One (128 + span)-row tile per 64-channel K chunk serves EVERY tap: tap t multiplies
 //                        rows [shift_t - shift_min, +128) of it through a row-shifted wgmma descriptor.  Rows outside [0, L) are
 //                        written as zeros = the convolution's zero padding.  Double-buffered.
-//   TMA warp             weight tiles [BN x 64] per (K chunk, tap) through a ring of mbarrier stages.
-//   MMA warpgroups (2)   wgmma M64 x BN x K16 each (the two 64-row halves of the tile), fp32 accumulator in registers; a finished
-//                        tile is stored to a shared-memory output tile while the registers already take the next one.
+//   TMA warp             (alone in its warpgroup) weight tiles [BN x 64] per (K chunk, tap) through a ring of mbarrier stages.
+//   MMA warpgroups (2)   wgmma M64 x BN x K16 each (the two 64-row halves of the tile), fp32 accumulator in registers, one
+//                        asynchronous wgmma group per tap step; a finished tile is stored to a shared-memory output tile while the
+//                        registers already take the next one.
 //   epilogue             output tile rows -> coalesced rows; bias / activation / channel scale / residual /
 //                        out_scale / accumulate / polyphase scatter fused; per-channel (sum, sumsq) of what was written is reduced in
 //                        shared memory and added to a float64 accumulator in global memory -- the NEXT layer's AdaIN statistics.
@@ -31,14 +33,27 @@ constexpr int TM = 128;
 constexpr int TK = 64;
 
 constexpr int MAXG = B2A_CONVF_MAX_PROBLEMS;
-// worker warps: every one converts A chunks AND runs epilogues (see the kernel's worker section).  Eight, not more: with the two MMA
-// warpgroups and the producer that is 17 warps, at most 5 on each of the SM's four schedulers, which leaves the 96 registers per thread
-// the N = 128 accumulator needs (21 warps would cap every thread at 80).
+// Roles sit on warpgroup boundaries because setmaxnreg re-allocates registers per warpgroup:
+//   warpgroups 0, 1  MMA            96 registers (the launch allocation: 64 accumulator + issue state)
+//   warpgroup 2      weight producer (warp 8, one lane; warps 9..11 idle)   32 registers (setmaxnreg.dec)
+//   warpgroups 3, 4  workers        128 registers (setmaxnreg.inc): A-chunk conversion AND epilogues (see the kernel's worker section)
+// 640 threads launch at 96 registers each (61 440 of the SM's 64 K); the producer's release of 64 x 128 covers the workers' 2 x 32 x 128.
 constexpr int NWORK = 8;
 constexpr int NSUB = NWORK / 4;                // workers per 32-row quarter: each takes every NSUB-th 32-column chunk
-constexpr int W_PROD = 8;                      // warps 0..7: the two MMA warpgroups; warp 8: weight producer; then the workers
-constexpr int W_WORK0 = 9;
-constexpr int THREADS = (W_WORK0 + NWORK) * 32;           // 544
+constexpr int WG_PROD = 2;
+constexpr int W_PROD = WG_PROD * 4;            // the producer warp
+constexpr int W_WORK0 = 12;                    // first worker warp (warpgroup 3)
+constexpr int THREADS = (W_WORK0 + NWORK) * 32;           // 640
+constexpr int REG_LAUNCH = 96;                 // 65536 / THREADS, rounded down to the allocation granule of 8
+constexpr int REG_MMA = 96, REG_PROD = 32, REG_WORK = 128;    // per-thread registers after re-allocation
+static_assert(THREADS % 128 == 0 && W_WORK0 % 4 == 0, "roles must sit on warpgroup boundaries");
+static_assert(2 * REG_MMA + REG_PROD + 2 * REG_WORK <= 5 * REG_LAUNCH, "the re-allocated registers must fit in the launch allocation");
+
+// Re-allocate this warpgroup's registers to R per thread (all 128 threads execute it).
+template <int R> __device__ __forceinline__ void set_regs() {
+  if constexpr (R < REG_LAUNCH) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+  else if constexpr (R > REG_LAUNCH) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 constexpr int RSTRIDE = NWORK * 32 / 16;                  // rows between a worker thread's consecutive A-tile rows (16 float4 slots per 64-channel row)
 constexpr int SACC = 4 * 2 * 128 * 4;                     // per-tile (sum, sumsq) partials: [32-row quarter][which][column <= 128]
 constexpr int CT_MAX = 1280;                              // channels of the per-CTA (scale, shift) table of the input transform
@@ -190,24 +205,38 @@ __device__ __forceinline__ void stats_coeffs(const FProb& P, int b, int c, float
   sh = (float)(be - s_ * mean);
 }
 
+// Per-tile control values of the MMA warpgroups.  The problem table lives in shared memory, and ptxas treats a shared-memory load as
+// possibly different per thread: a wgmma under a branch or loop bound taken from it sits on a "divergent path", and ptxas then
+// serialises every wgmma (warning C7520: each HGMMA waits for the one before it).  A shuffle from lane 0 is provably warp-uniform.
+struct MmaCtl { int kc0, kc1, taps, nb, two_w; };
+__device__ __forceinline__ MmaCtl mma_ctl(const FProb& P, const TileRef& t) {
+  const int kchunks = P.cin_pad / TK;
+  const int kc0 = t.ks * P.kper;
+  MmaCtl c;
+  c.kc0 = __shfl_sync(0xffffffffu, kc0, 0);
+  c.kc1 = __shfl_sync(0xffffffffu, min(kchunks, kc0 + P.kper), 0);
+  c.taps = __shfl_sync(0xffffffffu, P.taps, 0);
+  c.nb = __shfl_sync(0xffffffffu, P.BN >> 5, 0);
+  c.two_w = __shfl_sync(0xffffffffu, P.wplanes == 2, 0);
+  return c;
+}
+
 // One output tile on MMA warpgroup wg (threads 0..255): rows [64 wg, 64 wg + 64) of every K chunk x tap, accumulated in registers, then
-// stored to the shared-memory output tile once the workers have drained the previous one.  A ring slot / A buffer is handed back one
-// issue later (wgmma.wait_group 1).  Known limit: ptxas serialises these wgmmas (warning C7520; every HGMMA is followed by a wait) and
-// the kernel spills at its 96-register cap.  Selecting the hi/lo products at compile time removes C7520 but then reports C7512 (too few
-// registers) with more spills; a 13-warp layout (128 registers) and setmaxnreg re-allocation did not remove the spills either.  The
-// worker loops need the registers; the MMA work per K chunk is small next to the conversion, so the Kokoro step is not bound by it.
+// stored to the shared-memory output tile once the workers have drained the previous one.  Each tap step issues its products
+// (hi*hi, lo*hi, hi*lo), commits them as one group and waits only for the PREVIOUS step's group (wgmma.wait_group 1), whose ring slot /
+// A buffer is then handed back.  two_a comes from the kernel parameters (uniform), the rest from MmaCtl.  acc is the caller's one
+// 64-register accumulator, live across the tile loop, of which an NB variant uses the first NB * 16: with a separate array per variant
+// ptxas gives each its own register range (16 + 32 + 48 + 64 = 160 registers) and serialises the wgmmas for want of registers (C7512).
 template <int NB, bool F16>
-__device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const TileRef& t, uint32_t a0, uint32_t w0, uint64_t* full,
-                                         uint64_t* empty, uint64_t* a_full, uint64_t* a_empty, uint64_t* tfull, uint64_t* tempty,
+__device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const MmaCtl& c, bool two_a, float* acc, uint32_t a0, uint32_t w0,
+                                         uint64_t* full, uint64_t* empty, uint64_t* a_full, uint64_t* a_empty, uint64_t* tfull, uint64_t* tempty,
                                          float* acct, uint32_t lt, uint32_t& s, uint32_t& ph, uint32_t& cg) {
   const int wg = threadIdx.x >> 7;
   const bool leader = (threadIdx.x & 127) == 0;
-  float acc[NB * 16];
-  const int kchunks = P.cin_pad / TK;
-  const int kc0 = t.ks * P.kper, kc1 = min(kchunks, kc0 + P.kper);
-  const uint32_t wb = (uint32_t)P.BN * 128u, a_plane = (uint32_t)p.a_plane, a_buf = a_plane * (uint32_t)p.planes;
-  const bool two_a = p.planes == 2, two_w = P.wplanes == 2;
-  const int taps = P.taps, smin = P.shift_min;
+  const int kc0 = c.kc0, kc1 = c.kc1;
+  const uint32_t wb = (uint32_t)NB * 32u * 128u, a_plane = (uint32_t)p.a_plane, a_buf = a_plane * (two_a ? 2u : 1u);
+  const bool two_w = c.two_w != 0;
+  const int taps = c.taps, smin = P.shift_min;
   int pend_s = -1, pend_a = -1;
   uint32_t accum = 0;                                            // the tile's first MMA overwrites the accumulator
   for (int kc = kc0; kc < kc1; kc++, cg++) {
@@ -248,6 +277,31 @@ __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const
   if ((threadIdx.x & 31) == 0) mbar_arrive(tfull);               // 8 arrivals: the tile is complete
 }
 
+// Shared memory: [2] x A buffer (planes x a_plane bytes) | [wst] x W stage | output tile [128][acc_ld] | sacc | coefficient table | barriers.
+// Each role builds this after its setmaxnreg: pointers computed above the role split would be live into every role, and the 32-register
+// producer would spill them.
+struct SmemLayout {
+  int a_buf;
+  uint8_t* wbase;
+  float *acct, *sacc, *ctab_all;             // ctab_all: [slots][2][ct_stride] scale | shift of the input transform
+  uint64_t *full, *empty, *tfull, *tempty, *a_full, *a_empty;   // a_full / a_empty: [2]
+  int* flag_slot;
+  __device__ __forceinline__ SmemLayout(uint8_t* smem, const FParams& p) {
+    a_buf = p.a_plane * p.planes;
+    wbase = smem + (size_t)2 * a_buf;
+    acct = reinterpret_cast<float*>(wbase + (size_t)p.wst * p.w_stage);
+    sacc = acct + TM * p.acc_ld;
+    ctab_all = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sacc) + SACC);
+    full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ctab_all) + CTAB);
+    empty = full + p.wst;
+    tfull = empty + p.wst;
+    tempty = tfull + 1;
+    a_full = tempty + 1;
+    a_empty = a_full + 2;
+    flag_slot = reinterpret_cast<int*>(a_empty + 2);
+  }
+};
+
 // DBG = false compiles every timing stamp, wait accumulator and ablation flag out of the production kernel.
 template <bool DBG>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -271,24 +325,12 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
   __syncthreads();
   const FParams& p = sparams;
   if (threadIdx.x == 0) if (DBG) stamp(p, 0);
-  // layout: [2] x A buffer (planes x a_plane bytes) | [wst] x W stage | output tile [128][acc_ld] | sacc | coefficient table | barriers
-  const int a_buf = p.a_plane * p.planes;
-  uint8_t* wbase = smem + (size_t)2 * a_buf;
-  float* acct = reinterpret_cast<float*>(wbase + (size_t)p.wst * p.w_stage);
-  float* sacc = acct + TM * p.acc_ld;
-  float* ctab_all = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sacc) + SACC);  // [slots][2][ct_stride]: scale | shift of the input transform
-  uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ctab_all) + CTAB);
-  uint64_t* empty = full + p.wst;
-  uint64_t* tfull = empty + p.wst;
-  uint64_t* tempty = tfull + 1;
-  uint64_t* a_full = tempty + 1;             // [2]
-  uint64_t* a_empty = a_full + 2;            // [2]
-  int* flag_slot = reinterpret_cast<int*>(a_empty + 2);
 
   if (warp == W_PROD && lane == 0) {
-    for (int s = 0; s < p.wst; s++) { mbar_init(full + s, 1); mbar_init(empty + s, 2); }
-    mbar_init(tfull, 8); mbar_init(tempty, NWORK);
-    mbar_init(a_full, NWORK); mbar_init(a_full + 1, NWORK); mbar_init(a_empty, 2); mbar_init(a_empty + 1, 2);
+    const SmemLayout sl(smem, p);
+    for (int s = 0; s < p.wst; s++) { mbar_init(sl.full + s, 1); mbar_init(sl.empty + s, 2); }
+    mbar_init(sl.tfull, 8); mbar_init(sl.tempty, NWORK);
+    mbar_init(sl.a_full, NWORK); mbar_init(sl.a_full + 1, NWORK); mbar_init(sl.a_empty, 2); mbar_init(sl.a_empty + 1, 2);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -296,9 +338,16 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
   if (threadIdx.x == 0) if (DBG) stamp(p, 1);
   pdl_launch_dependents();        // the next kernel may start its own prologue / weight loads as SMs free up; it waits for us before reading
 
-  if (warp == W_PROD) {
+  // warpgroup index through a shuffle: provably uniform, so ptxas sees each role (and the wgmmas inside it) on a non-divergent path
+  const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  if (wgi == WG_PROD) {
     // ===== weight producer: independent of the previous kernel's output, so it starts before the programmatic-dependency wait =====
-    if (lane == 0) {
+    set_regs<REG_PROD>();
+    if (warp == W_PROD && lane == 0) {
+      const SmemLayout sl(smem, p);
+      uint8_t* const wbase = sl.wbase;
+      uint64_t* const full = sl.full;
+      uint64_t* const empty = sl.empty;
       const CUtensorMap* mws[MAXG] = {&mw0, &mw1, &mw2, &mw3};
       const CUtensorMap* mls[MAXG] = {&ml0, &ml1, &ml2, &ml3};
       for (int g = 0; g < p.G; g++) {
@@ -328,16 +377,26 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
       }
       if (DBG && p.dbg) { p.dbg[(size_t)blockIdx.x * 32 + 21] = (unsigned long long)(clock64() - pt0); p.dbg[(size_t)blockIdx.x * 32 + 22] = w_pempty; }
     }
-  } else if (warp < W_PROD) {
+  } else if (wgi < WG_PROD) {
     // ===== MMA warpgroups =====
-    const uint32_t a0 = smem_u32(smem), w0 = smem_u32(wbase);
+    set_regs<REG_MMA>();
+    const SmemLayout sl(smem, p);
+    uint64_t *const full = sl.full, *const empty = sl.empty, *const a_full = sl.a_full, *const a_empty = sl.a_empty;
+    uint64_t *const tfull = sl.tfull, *const tempty = sl.tempty;
+    float* const acct = sl.acct;
+    const uint32_t a0 = smem_u32(smem), w0 = smem_u32(sl.wbase);
+    const bool f16 = gp.f16 != 0, two_a = gp.planes == 2;       // kernel parameters: uniform
     uint32_t s = 0, ph = 0, lt = 0, cg = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, lt++) {
+    float acc[4 * 16];                                          // shared by every NB variant (see mma_tile)
+#pragma unroll
+    for (int i = 0; i < 4 * 16; i++) acc[i] = 0.f;
+    for (int tile = blockIdx.x; tile < gp.ntiles; tile += gridDim.x, lt++) {
       const TileRef t = decode_tile(p, tile);
       const FProb& P = p.pr[t.g];
-#define B2A_MMA_TILE(NB) (p.f16 ? mma_tile<NB, true>(p, P, t, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg) \
-                                : mma_tile<NB, false>(p, P, t, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg))
-      switch (P.BN >> 5) {
+      const MmaCtl c = mma_ctl(P, t);
+#define B2A_MMA_TILE(NB) (f16 ? mma_tile<NB, true>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg) \
+                              : mma_tile<NB, false>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg))
+      switch (c.nb) {
         case 1: B2A_MMA_TILE(1); break;
         case 2: B2A_MMA_TILE(2); break;
         case 3: B2A_MMA_TILE(3); break;
@@ -347,6 +406,12 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
     }
   } else {
     // ===== worker warps: A-tile conversion AND epilogue =====
+    set_regs<REG_WORK>();
+    const SmemLayout sl(smem, p);
+    const int a_buf = sl.a_buf;
+    float *const acct = sl.acct, *const sacc = sl.sacc, *const ctab_all = sl.ctab_all;
+    uint64_t *const a_full = sl.a_full, *const a_empty = sl.a_empty, *const tfull = sl.tfull, *const tempty = sl.tempty;
+    int* const flag_slot = sl.flag_slot;
     // The first version of this kernel split the roles (8 converter + 8 epilogue warps).  Its profile on the Kokoro layers: the converter
     // was the bottleneck everywhere (~5 us per K chunk, issue-latency bound with two warps per scheduler) while the epilogue warps
     // idled ~70 % of the time, and the two big loops evicted each other from the instruction caches (a third of the stall samples
