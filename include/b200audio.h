@@ -101,7 +101,14 @@ int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16, int32_t B
                       int32_t post_act, float post_p0, const float* cscale, int64_t cscale_bs, const float* res,
                       int64_t res_bs, int64_t res_ld, int32_t res_div, float out_scale, int32_t accumulate, float* y,
                       int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop, double* stats_ws,
-                      int32_t stats_slots, void* stream);
+                      int32_t stats_slots, void* emit_hi, void* emit_lo, int64_t emit_ld, void* attn_ws, int32_t attn_heads,
+                      float attn_scale, void* stream);
+/* b2a_conv1d_tc also writes its consumer's A operand from the epilogue (up_stride == 0 only; at most one of the two):
+ *   emit_hi != NULL: bf16 planes bf16(y), bf16(y - hi) [B, Lout, emit_ld] (lo == NULL: hi only) -- what b2a_prep_bf16 makes of y;
+ *   attn_ws != NULL: y is a fused [q | k | v] projection (Cout = 3 * 64 * attn_heads) and the epilogue fills b2a_attention_tc's
+ *   workspace attn_ws (Tq = Tk = Lout, scale attn_scale) as its prologue would; then call it with operands_ready = 1.
+ * The N tile is the widest divisor of Cout up to 128 unless that grid covers under half the SMs; then the widest whose grid still
+ * covers them all (or 32).  Launched with programmatic dependent launch: weight tiles are fetched before the dependency wait. */
 
 /* profiling aid: CTA (0,0,0) of subsequent b2a_conv1d_tc launches stamps clock64() at its phase boundaries into dbg8[0..6]
  * (entry, setup done, first operands landed, last operands landed, accumulator ready, epilogue done, exit); NULL disables. */
@@ -145,7 +152,9 @@ int32_t b2a_coeffs_from_stats(const int64_t* stats, int32_t B, int32_t L, int32_
  * (nn.LayerNorm, modules.py:71-90 AdaLayerNorm). rms != 0 -> RMSNorm (no mean, talker.py:267). */
 int32_t b2a_layernorm(const float* x, int64_t x_ld, const float* res, int64_t res_ld, float* y, int64_t y_ld,
                       int64_t rows, int32_t C, const float* w, const float* b, const float* ada, float eps,
-                      int32_t rms, int32_t post_act, float post_p0, void* stream);
+                      int32_t rms, int32_t post_act, float post_p0, void* emit_hi, void* emit_lo, int64_t emit_ld, void* stream);
+/* emit_hi != NULL: also the bf16 planes bf16(y), bf16(y - hi) of every row, [rows, emit_ld] (lo may be NULL) -- the next GEMM's
+ * A operand, as b2a_prep_bf16 would make it.  Needs C % 8 == 0, C <= 1024 and 16-byte aligned rows. */
 
 /* ---- attention -----------------------------------------------------------------------------
  * softmax(scale * q k^T + mask) v with fp32 softmax; replaces mx.fast.scaled_dot_product_attention
@@ -158,11 +167,15 @@ typedef struct {
   int32_t B, Tq, Tk, H, Hkv, D;
   float scale; int32_t causal, q_offset, window;
   const int32_t* k_len;     /* [B] valid key count or NULL */
+  /* b2a_attention_tc only: */
+  void* emit_hi; void* emit_lo; int64_t emit_ld;   /* optional bf16 planes bf16(o), bf16(o - hi) [B, Tq, emit_ld] for the next GEMM */
+  int32_t operands_ready;   /* != 0: ws already holds the q / k / v planes (b2a_conv1d_tc's attention-operand epilogue); q, k, v unused */
 } b2a_attn_t;
 int32_t b2a_attention(const b2a_attn_t* p, void* stream);
 /* Same contract on the tensor cores (wgmma) for D == 64, H == Hkv, k_len == NULL: S = QK^T and PV as fp16 hi/lo-plane MMAs
  * (fp32-grade products), online softmax with one thread per query row.  ws: device scratch of b2a_attention_tc_ws_bytes bytes
- * (fp16 planes of q, k and the transposed v). */
+ * (fp16 planes of q * scale * log2(e), k and the transposed v, keys zero-padded to a multiple of 8).  Launched with programmatic
+ * dependent launch. */
 int64_t b2a_attention_tc_ws_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk);
 int32_t b2a_attention_tc(const b2a_attn_t* p, void* ws, void* stream);
 /* in-place rotary embedding on x [B,T,H,D] (token stride ld): traditional != 0 rotates pairs (2i,2i+1)

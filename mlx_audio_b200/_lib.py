@@ -40,6 +40,7 @@ class AttnParams(C.Structure):
         ("B", i32), ("Tq", i32), ("Tk", i32), ("H", i32), ("Hkv", i32), ("D", i32),
         ("scale", f32), ("causal", i32), ("q_offset", i32), ("window", i32),
         ("k_len", C.c_void_p),
+        ("emit_hi", C.c_void_p), ("emit_lo", C.c_void_p), ("emit_ld", i64), ("operands_ready", i32),
     ]
 
 
@@ -69,7 +70,7 @@ PROTOTYPES = {
     "b2a_convtr1d_cl": (i32, [C.POINTER(Conv1dParams), C.c_void_p]),
     "b2a_prep_bf16": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, i32, f32, c_f, c_f, c_f, c_f, i32, C.c_void_p]),
     "b2a_conv1d_tc": (i32, [c_f, c_f, i32, i32, i32, i32, c_f, c_f, i32, C.POINTER(i32), i32, i32, c_f, i32, f32, c_f, i64, c_f, i64, i64, i32, f32, i32,
-                            c_f, i64, i64, i32, i32, c_f, i32, C.c_void_p]),
+                            c_f, i64, i64, i32, i32, c_f, i32, c_f, c_f, i64, c_f, i32, f32, C.c_void_p]),
     "b2a_conv1d_tc_debug": (i32, [c_f]),
     "b2a_conv1d_fused_debug": (i32, [c_f]),
     "b2a_conv1d_fused": (i32, [C.POINTER(ConvFParams), i32, i32, i32, c_f, i64, C.c_void_p]),
@@ -81,7 +82,7 @@ PROTOTYPES = {
     "b2a_adain_coeffs_from_partials": (i32, [c_f, i32, i32, i32, i32, c_f, f32, c_f, c_f, C.c_void_p]),
     "b2a_channel_stats": (i32, [c_f, i64, i64, i32, i32, i32, C.POINTER(C.c_void_p), C.POINTER(i64), i32, C.c_void_p]),
     "b2a_coeffs_from_stats": (i32, [c_f, i32, i32, i32, c_f, f32, c_f, c_f, C.c_void_p]),
-    "b2a_layernorm": (i32, [c_f, i64, c_f, i64, c_f, i64, i64, i32, c_f, c_f, c_f, f32, i32, i32, f32, C.c_void_p]),
+    "b2a_layernorm": (i32, [c_f, i64, c_f, i64, c_f, i64, i64, i32, c_f, c_f, c_f, f32, i32, i32, f32, c_f, c_f, i64, C.c_void_p]),
     "b2a_attention": (i32, [C.POINTER(AttnParams), C.c_void_p]),
     "b2a_attention_tc_ws_bytes": (i64, [i32, i32, i32, i32]),
     "b2a_attention_tc": (i32, [C.POINTER(AttnParams), C.c_void_p, C.c_void_p]),

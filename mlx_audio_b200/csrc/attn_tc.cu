@@ -46,6 +46,7 @@ struct AtcParams {
   int B, H, Tq, Tk;
   int causal, q_offset, window;
   float* o; int64_t o_bs, o_ld;          // [B, Tq, H*64] fp32
+  __nv_bfloat16 *e_hi, *e_lo; int64_t e_ld;   // optional bf16 hi / lo planes of o, [B, Tq, e_ld] (the next GEMM's A operand)
 };
 
 // ---- prologue: fp32 [B,T,H*64] -> fp16 hi/lo planes.  q,k: [B*H, T, 64];  v: transposed [B*H, 64, Tkp] (zero-padded keys)
@@ -61,7 +62,7 @@ __global__ void attn_tc_prep_qk_kernel(const float* x, int64_t x_bs, int64_t x_l
     float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
     __align__(16) __half hh[8], ll[8];
 #pragma unroll
-    for (int j = 0; j < 8; j++) { float f = v[j] * mul; hh[j] = __float2half_rn(f); ll[j] = __float2half_rn(f - __half2float(hh[j])); }
+    for (int j = 0; j < 8; j++) split16(v[j] * mul, hh[j], ll[j]);
     const int64_t dst = (((int64_t)b * H + h) * T + t) * HD + c8 * 8;
     *reinterpret_cast<uint4*>(hi + dst) = *reinterpret_cast<uint4*>(hh);
     *reinterpret_cast<uint4*>(lo + dst) = *reinterpret_cast<uint4*>(ll);
@@ -82,10 +83,10 @@ __global__ void attn_tc_prep_vt_kernel(const float* v, int64_t v_bs, int64_t v_l
     const int tt = i & 63, d = i >> 6;
     const int t = t0 + tt;
     if (t < Tp) {
-      const float f = tile[tt][d];
-      const __half hh = __float2half_rn(f);
+      __half hh, ll;
+      split16(tile[tt][d], hh, ll);
       hi[(base + d) * Tp + t] = hh;
-      lo[(base + d) * Tp + t] = __float2half_rn(f - __half2float(hh));
+      lo[(base + d) * Tp + t] = ll;
     }
   }
 }
@@ -123,6 +124,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
+  pdl_wait();                                                    // the operand planes are the predecessor's output
 
   if (warp == 8) {
     if (lane == 0 && nt > 0) {
@@ -235,6 +237,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
     for (int j = 0; j < 32; j++) o[j] = fmaf(o[j], alpha[(j >> 1) & 1], pv[j]);
     if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + s);     // both warpgroups release the stage
   }
+  pdl_launch_dependents();
   // ---- write out: a quad of lanes covers 8 consecutive columns (32 B) of a row
   float inv[2];
 #pragma unroll
@@ -252,6 +255,17 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
 #pragma unroll
       for (int j = 0; j < 8; j++)
         *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * h] * inv[h], o[4 * j + 2 * h + 1] * inv[h]);
+      if (p.e_hi) {
+        const int64_t e = ((int64_t)b * p.Tq + q) * p.e_ld + hh * HD + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          __nv_bfloat162 eh, el;
+          split16(o[4 * j + 2 * h] * inv[h], eh.x, el.x);
+          split16(o[4 * j + 2 * h + 1] * inv[h], eh.y, el.y);
+          *reinterpret_cast<__nv_bfloat162*>(p.e_hi + e + 8 * j) = eh;
+          if (p.e_lo) *reinterpret_cast<__nv_bfloat162*>(p.e_lo + e + 8 * j) = el;
+        }
+      }
     }
   }
 }
@@ -274,29 +288,29 @@ int map3(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint64_t d2
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-inline int64_t tk_pad(int Tk) { return ((int64_t)Tk + 7) / 8 * 8; }
-
 }  // namespace
 
 extern "C" int64_t b2a_attention_tc_ws_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk) {
   const int64_t bh = (int64_t)B * H;
-  return 2 * 2 * (bh * Tq * HD + bh * Tk * HD + bh * HD * tk_pad(Tk)) + 1024;
+  return 2 * 2 * (bh * Tq * HD + bh * Tk * HD + bh * HD * (((int64_t)Tk + 7) / 8 * 8)) + 1024;
 }
 
 extern "C" int32_t b2a_attention_tc(const b2a_attn_t* a, void* ws, void* stream) {
-  B2A_CHECK_ARG(a && ws && a->q && a->k && a->v && a->o, "null pointer");
+  B2A_CHECK_ARG(a && ws && a->o && (a->operands_ready || (a->q && a->k && a->v)), "null pointer");
   B2A_CHECK_ARG(a->D == 64 && a->H == a->Hkv && a->k_len == nullptr, "tensor-core attention: head_dim 64, no GQA, no per-row key length");
   B2A_CHECK_ARG(a->B > 0 && a->Tq > 0 && a->Tk > 0 && a->H > 0, "bad shape");
-  B2A_CHECK_ARG(a->q_ld % 4 == 0 && a->k_ld % 4 == 0 && a->o_ld % 4 == 0 && a->q_bs % 4 == 0 && a->k_bs % 4 == 0 && a->o_bs % 4 == 0 &&
-                ((uintptr_t)a->q & 15) == 0 && ((uintptr_t)a->k & 15) == 0 && ((uintptr_t)a->o & 15) == 0, "q/k/o rows must be 16-byte aligned");
+  B2A_CHECK_ARG(a->operands_ready ||
+                (a->q_ld % 4 == 0 && a->k_ld % 4 == 0 && a->q_bs % 4 == 0 && a->k_bs % 4 == 0 && ((uintptr_t)a->q & 15) == 0 && ((uintptr_t)a->k & 15) == 0),
+                "q/k rows must be 16-byte aligned");
+  B2A_CHECK_ARG(a->o_ld % 4 == 0 && a->o_bs % 4 == 0 && ((uintptr_t)a->o & 15) == 0, "o rows must be 16-byte aligned");
+  B2A_CHECK_ARG(!a->emit_hi || (a->emit_ld >= a->H * HD && a->emit_ld % 8 == 0), "emitted planes: row stride >= H*64, a multiple of 8");
   cudaStream_t st = (cudaStream_t)stream;
   const int B = a->B, H = a->H, Tq = a->Tq, Tk = a->Tk;
-  const int64_t bh = (int64_t)B * H, Tkp = tk_pad(Tk);
-  __half* base = (__half*)(((uintptr_t)ws + 255) & ~(uintptr_t)255);
-  __half* qh = base; __half* ql = qh + bh * Tq * HD;
-  __half* kh = ql + bh * Tq * HD; __half* kl = kh + bh * Tk * HD;
-  __half* vh = kl + bh * Tk * HD; __half* vl = vh + bh * HD * Tkp;
-  {
+  const int64_t bh = (int64_t)B * H;
+  const AttnOperands op = attn_operands(ws, bh, Tq, Tk);
+  __half *qh = op.qh, *ql = op.ql, *kh = op.kh, *kl = op.kl, *vh = op.vh, *vl = op.vl;
+  const int64_t Tkp = op.tkp;
+  if (!a->operands_ready) {
     int64_t tq = bh * Tq * (HD / 8), tk = bh * Tk * (HD / 8);
     int gq = (int)((tq + 255) / 256); if (gq > 132 * 16) gq = 132 * 16;
     int gk = (int)((tk + 255) / 256); if (gk > 132 * 16) gk = 132 * 16;
@@ -313,11 +327,14 @@ extern "C" int32_t b2a_attention_tc(const b2a_attn_t* a, void* ws, void* stream)
   if (!e) e = map3(&mvh, vh, Tkp, HD, bh, Tkp * 2, (uint64_t)HD * Tkp * 2, BN, HD);
   if (!e) e = map3(&mvl, vl, Tkp, HD, bh, Tkp * 2, (uint64_t)HD * Tkp * 2, BN, HD);
   if (e) { b2a_set_error("b2a_attention_tc: cuTensorMapEncodeTiled failed (%d)", e); return B2A_E_CUDA; }
-  AtcParams p{B, H, Tq, Tk, a->causal, a->q_offset, a->window, a->o, a->o_bs, a->o_ld};
+  AtcParams p{B, H, Tq, Tk, a->causal, a->q_offset, a->window, a->o, a->o_bs, a->o_ld,
+              (__nv_bfloat16*)a->emit_hi, (__nv_bfloat16*)a->emit_lo, a->emit_ld};
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); attr = true; }
   dim3 grid((Tq + BM - 1) / BM, (unsigned)bh);
-  attn_tc_kernel<<<grid, THREADS, SMEM_BYTES, st>>>(mqh, mql, mkh, mkl, mvh, mvl, p);
-  B2A_CHECK_LAUNCH();
+  if (b2a_launch_pdl(attn_tc_kernel, grid, dim3(THREADS), SMEM_BYTES, st, mqh, mql, mkh, mkl, mvh, mvl, p) != cudaSuccess) {
+    b2a_set_error("b2a_attention_tc: %s", cudaGetErrorString(cudaGetLastError()));
+    return B2A_E_CUDA;
+  }
   return B2A_OK;
 }

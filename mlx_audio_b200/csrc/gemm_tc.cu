@@ -42,7 +42,42 @@ struct TcParams {
   float* y; int64_t y_bs, y_ld;
   long long* dbg;                 // optional: clock64 stamps from CTA (0,0,0) (b2a_conv1d_tc_debug)
   double* stats; int stats_slots; // optional InstanceNorm partials of the OUTPUT: [B][stats_slots][C][2] = (sum, sum of squares) per 32-row group
+  // optional: the consumer's A operand, split16 of each final value y.  Either bf16 planes [B][Lout][e_ld] of the next GEMM, or (attn.qh
+  // != null) the fp16 attention operands of a fused qkv projection: column n = part * a_hs + head * 64 + d, part 0 = Q (times a_qmul),
+  // 1 = K, 2 = V (transposed, keys zero-padded to attn.tkp).
+  __nv_bfloat16 *e_hi, *e_lo; int64_t e_ld;
+  AttnOperands attn; int a_H, a_hs; float a_qmul;
 };
+
+// Where this lane's column of the output tile goes as split16 planes: hi / lo pointers at row 0 of batch b, and the element step per row.
+struct EmitCol { uint16_t *hi, *lo; int64_t step; float mul; bool f16; };
+__device__ __forceinline__ EmitCol emit_col(const TcParams& p, int b, int n) {
+  EmitCol c{nullptr, nullptr, 0, 1.f, false};
+  if (p.attn.qh) {
+    const int part = n / p.a_hs, head = (n - part * p.a_hs) >> 6, d = n & 63;
+    const int64_t bh = (int64_t)b * p.a_H + head;
+    c.f16 = true;
+    if (part < 2) {
+      const int64_t o = bh * p.Lout * 64 + d;
+      c.hi = (uint16_t*)(part ? p.attn.kh : p.attn.qh) + o; c.lo = (uint16_t*)(part ? p.attn.kl : p.attn.ql) + o;
+      c.step = 64; c.mul = part ? 1.f : p.a_qmul;
+    } else {
+      const int64_t o = (bh * 64 + d) * p.attn.tkp;
+      c.hi = (uint16_t*)p.attn.vh + o; c.lo = (uint16_t*)p.attn.vl + o; c.step = 1;
+    }
+  } else if (p.e_hi) {
+    const int64_t o = (int64_t)b * p.Lout * p.e_ld + n;
+    c.hi = (uint16_t*)p.e_hi + o; c.lo = p.e_lo ? (uint16_t*)p.e_lo + o : nullptr; c.step = p.e_ld;
+  }
+  return c;
+}
+__device__ __forceinline__ void emit_store(const EmitCol& c, int64_t row, float v) {
+  uint16_t h, l;
+  if (c.f16) { __half a, b; split16(v * c.mul, a, b); h = __half_as_ushort(a); l = __half_as_ushort(b); }
+  else { __nv_bfloat16 a, b; split16(v, a, b); h = __bfloat16_as_ushort(a); l = __bfloat16_as_ushort(b); }
+  c.hi[row * c.step] = h;
+  if (c.lo) c.lo[row * c.step] = l;
+}
 
 // smem: [stages] x { A_hi 16 KB | A_lo 16 KB (planes==2) | W BN*128 B (x wplanes) }, then barriers.  After the K loop the stage
 // memory holds the 128 x (BN + 8) fp32 output tile (row stride = 8 mod 32 words: the fragment stores of a quarter-warp hit distinct banks).
@@ -83,20 +118,34 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
   if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
+      // The weights never depend on the preceding kernel: the first ring's weight tiles are in flight before the programmatic
+      // dependency wait, and each of those stages' A tiles joins the same transaction count after it.
+      const int pre = iters < p.stages ? iters : p.stages;
+      for (int it = 0; it < pre; it++) {
+        const int tap = it / kchunks, kc = it % kchunks;
+        uint8_t* st = smem + (size_t)it * stage_bytes;
+        mbar_expect_tx(full + it, (uint32_t)stage_bytes);
+        tma_load_2d(st + (size_t)a_bytes * p.planes, &map_w, full + it, kc * TK, tap * p.Cout + n0);
+        if (p.wplanes == 2) tma_load_2d(st + (size_t)a_bytes * p.planes + w_bytes, &map_wlo, full + it, kc * TK, tap * p.Cout + n0);
+      }
+      pdl_wait();
       for (int it = 0; it < iters; it++) {
         const int s = it % p.stages, ph = (it / p.stages) & 1;
-        mbar_wait(empty + s, ph ^ 1);
         const int tap = it / kchunks, kc = it % kchunks;
         uint8_t* st = smem + (size_t)s * stage_bytes;
-        mbar_expect_tx(full + s, (uint32_t)stage_bytes);
+        if (it >= pre) {
+          mbar_wait(empty + s, ph ^ 1);
+          mbar_expect_tx(full + s, (uint32_t)stage_bytes);
+          tma_load_2d(st + (size_t)a_bytes * p.planes, &map_w, full + s, kc * TK, tap * p.Cout + n0);
+          if (p.wplanes == 2) tma_load_2d(st + (size_t)a_bytes * p.planes + w_bytes, &map_wlo, full + s, kc * TK, tap * p.Cout + n0);
+        }
         tma_load_3d(st, &map_hi, full + s, kc * TK, l0 + p.shift[tap], b);
         if (p.planes == 2) tma_load_3d(st + a_bytes, &map_lo, full + s, kc * TK, l0 + p.shift[tap], b);
-        tma_load_2d(st + (size_t)a_bytes * p.planes, &map_w, full + s, kc * TK, tap * p.Cout + n0);
-        if (p.wplanes == 2) tma_load_2d(st + (size_t)a_bytes * p.planes + w_bytes, &map_wlo, full + s, kc * TK, tap * p.Cout + n0);
       }
     }
     return;
   }
+  pdl_wait();                                              // the epilogue reads res / y and writes y: after the predecessor
 
   // ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the tile =====
   const int wg = warp >> 2;
@@ -125,6 +174,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
     wgmma_wait<0>();
     wgmma_fence_regs<NB * 16>(acc);
   }
+  pdl_launch_dependents();
   // both warpgroups are done reading the operand ring (and every TMA write to it has landed): it becomes the output tile
   bar_sync(1, 256);
   float* tile = reinterpret_cast<float*>(smem);
@@ -169,6 +219,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
     const float* rp = rcol ? rcol + (int64_t)(half_res ? (row0 >> 1) : row0) * p.res_ld : nullptr;
     const int64_t rstride = (int64_t)mul * p.res_ld;
     const float osc = p.out_scale;
+    const EmitCol ec = emit_col(p, b, n);                  // up-sampling mode never emits (host check), so row = row0 + i below
     float st1 = 0.f, st2 = 0.f;                            // InstanceNorm partials of the values written below (this lane's column)
     if (i_lo == 0 && i_hi == 32) {
       float rr[32];
@@ -200,12 +251,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
         for (int i = 0; i < 32; i++) {
           const float v = act_noinline(stage[i * LD + lane] + bias, p.post_act, p.post_p0) * cso + rr[i];
           yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
+          if (ec.hi) emit_store(ec, row0 + i, v);
         }
       } else {
 #pragma unroll
         for (int i = 0; i < 32; i++) {
           const float v = (stage[i * LD + lane] + bias) * cso + rr[i];
           yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
+          if (ec.hi) emit_store(ec, row0 + i, v);
         }
       }
     } else {
@@ -217,7 +270,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
         float o = p.accumulate ? ycol[(int64_t)row * p.y_ld] : 0.f;
         const float v = (t * cs + rv) * osc + o;
         ycol[(int64_t)row * p.y_ld] = v; st1 += v; st2 = fmaf(v, v, st2);
+        if (ec.hi) emit_store(ec, row, v);
       }
+      // transposed V: the zero keys that pad Lout to attn.tkp (< 8 rows past the last valid one, so inside this ragged chunk)
+      if (ec.hi && ec.step == 1)
+        for (int64_t row = p.Lout; row < p.attn.tkp; row++) { ec.hi[row] = 0; ec.lo[row] = 0; }
     }
     if (p.stats) {
       double* w = p.stats + ((((int64_t)b * p.stats_slots + (int64_t)(mt * 4 + quarter) * mul + ph) * p.C) + co) * 2;
@@ -228,12 +285,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
 }
 
 // ---- prologue: fp32 activations -> (hi, lo) bf16 planes with the fused input transform; pad channels are zeroed
-template <typename T> __device__ __forceinline__ T to16(float v);
-template <> __device__ __forceinline__ __nv_bfloat16 to16<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-template <> __device__ __forceinline__ __half to16<__half>(float v) { return __float2half_rn(v); }
-__device__ __forceinline__ float from16(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float from16(__half v) { return __half2float(v); }
-
 // 8 channels per thread: 2 x 16-byte reads, one 16-byte write per plane
 // ACT >= 0: the activation is a compile-time constant (no per-element switch, a third of the code: the generic instantiation was
 // instruction-cache- and branch-bound); ACT = -1: runtime `act`.
@@ -276,8 +327,7 @@ __global__ void prep_bf16_kernel(const float* __restrict__ x, int64_t x_bs, int6
         else if constexpr (ACT == 0) { }
         else if (act) t = b2a_act(t, act, p0, a ? __ldg(a + cc) : 1.f, bb ? __ldg(bb + cc) : 1.f);
       }
-      h[q] = to16<T16>(t);
-      lw[q] = to16<T16>(t - from16(h[q]));
+      split16(t, h[q], lw[q]);
     }
     *reinterpret_cast<uint4*>(hi + r * cpad + c) = *reinterpret_cast<uint4*>(h);
     if (lo) *reinterpret_cast<uint4*>(lo + r * cpad + c) = *reinterpret_cast<uint4*>(lw);
@@ -340,8 +390,12 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
                                  int32_t post_act, float post_p0, const float* cscale, int64_t cscale_bs, const float* res,
                                  int64_t res_bs, int64_t res_ld, int32_t res_div, float out_scale, int32_t accumulate, float* y,
                                  int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop, double* stats_ws, int32_t stats_slots,
+                                 void* emit_hi, void* emit_lo, int64_t emit_ld, void* attn_ws, int32_t attn_heads, float attn_scale,
                                  void* stream) {
   B2A_CHECK_ARG(a_hi && w_bf16 && y && shifts_host, "null pointer");
+  B2A_CHECK_ARG(!(emit_hi && attn_ws) && (!(emit_hi || attn_ws) || up_stride == 0), "one emitted operand at most, not in transposed mode");
+  B2A_CHECK_ARG(!emit_hi || (emit_ld >= Cout && emit_ld % 8 == 0), "emitted planes: row stride >= Cout, a multiple of 8");
+  B2A_CHECK_ARG(!attn_ws || (attn_heads > 0 && Cout == 3 * 64 * attn_heads), "attention operands: Cout = 3 * 64 * heads (q | k | v)");
   B2A_CHECK_ARG(up_stride >= 0 && up_crop >= 0 && (up_stride == 0 || (Cout % up_stride == 0 && (Cout / up_stride) % 32 == 0)),
                 "transposed mode: Cout = up_stride * C with C a multiple of 32");
   B2A_CHECK_ARG(B > 0 && L > 0 && Lout > 0 && taps > 0 && taps <= 32 && cin_pad % 64 == 0 && (res_div == 1 || res_div == 2), "bad shape (res_div must be 1 or 2)");
@@ -357,7 +411,22 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
   // the Qwen3 vocoder's 96-, 192- and 384-channel blocks would otherwise run as 32-/64-wide tiles and re-read A three times.
   p.BN = 32;
   for (int bn = BN_MAX; bn >= 32; bn -= 32) if (Cout % bn == 0) { p.BN = bn; break; }
+  // Few-row GEMMs (ALBERT at T = 130: 2 row tiles) leave most SMs idle at that width and every CTA runs the whole K loop alone:
+  // when the grid covers under half the SMs, take the widest tile whose grid still reaches the SM count, else the narrowest (32).
+  // Each output element still accumulates its whole K range in the same order inside one CTA.
+  static int nsm = 0;
+  if (!nsm) { nsm = b2a_device_sm_count(); if (nsm <= 0) nsm = 132; }
+  const int64_t row_tiles = (int64_t)cdiv(p.Mrows, TM) * B;
+  if (row_tiles * (Cout / p.BN) * 2 < nsm) {
+    int bn = 32;
+    for (int c = p.BN; c > 32; c -= 32) if (Cout % c == 0 && row_tiles * (Cout / c) >= nsm) { bn = c; break; }
+    p.BN = bn;
+  }
   for (int i = 0; i < taps; i++) p.shift[i] = shifts_host[i];
+  p.e_hi = (__nv_bfloat16*)emit_hi; p.e_lo = (__nv_bfloat16*)emit_lo; p.e_ld = emit_ld;
+  p.attn = attn_ws ? attn_operands(attn_ws, (int64_t)B * attn_heads, Lout, Lout) : AttnOperands{};
+  p.a_H = attn_heads; p.a_hs = attn_heads * 64;
+  p.a_qmul = attn_scale * 1.4426950408889634f;            // as b2a_attention_tc pre-scales Q: exp2 is its only transcendental
   p.bias = bias; p.post_act = post_act; p.post_p0 = post_p0; p.cscale = cscale; p.cscale_bs = cscale_bs;
   p.res = res; p.res_bs = res_bs; p.res_ld = res_ld; p.res_div = res_div; p.out_scale = out_scale; p.accumulate = accumulate;
   p.y = y; p.y_bs = y_bs; p.y_ld = y_ld;
@@ -407,7 +476,9 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
     attr = true;
   }
   dim3 grid(cdiv(p.Mrows, TM), Cout / p.BN, B);
-  kernels[p.f16][p.BN / 32 - 1]<<<grid, THREADS, smem, (cudaStream_t)stream>>>(mh, ml, mw, mwl, p);
-  B2A_CHECK_LAUNCH();
+  if (b2a_launch_pdl(kernels[p.f16][p.BN / 32 - 1], grid, dim3(THREADS), smem, (cudaStream_t)stream, mh, ml, mw, mwl, p) != cudaSuccess) {
+    b2a_set_error("b2a_conv1d_tc: %s", cudaGetErrorString(cudaGetLastError()));
+    return B2A_E_CUDA;
+  }
   return B2A_OK;
 }

@@ -3,6 +3,7 @@
 // so that var = E[x^2] - mean^2 stays exact for long sequences; the normalisation itself is
 // applied for free inside the consuming conv's prologue (conv.cu: Pre).
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace {
 
@@ -127,7 +128,9 @@ template <int NV>
 __global__ void __launch_bounds__(128) layernorm_vec_kernel(const float* __restrict__ x, int64_t x_ld, const float* __restrict__ res, int64_t res_ld,
                                                             float* __restrict__ y, int64_t y_ld, int64_t rows, int C, const float* __restrict__ w,
                                                             const float* __restrict__ bb, const float* __restrict__ ada, float eps, int rms,
-                                                            int post_act, float post_p0) {
+                                                            int post_act, float post_p0, __nv_bfloat16* __restrict__ e_hi,
+                                                            __nv_bfloat16* __restrict__ e_lo, int64_t e_ld) {
+  pdl_wait();                                              // x / res are the preceding kernel's output
   const int64_t row = (int64_t)blockIdx.x * 4 + threadIdx.x / 32;
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -162,6 +165,7 @@ __global__ void __launch_bounds__(128) layernorm_vec_kernel(const float* __restr
   }
   s2 = warp_sum(s2);
   const float rstd = rsqrtf(s2 / C + eps);
+  pdl_launch_dependents();
   float4* yp = reinterpret_cast<float4*>(y + row * y_ld);
 #pragma unroll
   for (int j = 0; j < NV; j++) {
@@ -176,6 +180,13 @@ __global__ void __launch_bounds__(128) layernorm_vec_kernel(const float* __restr
         if (post_act) o[q] = b2a_act(o[q], post_act, post_p0, 1.f, 1.f);
       }
       yp[i] = make_float4(o[0], o[1], o[2], o[3]);
+      if (e_hi) {
+        __align__(8) __nv_bfloat16 h[4], l[4];
+#pragma unroll
+        for (int q = 0; q < 4; q++) tc::split16(o[q], h[q], l[q]);
+        *reinterpret_cast<uint2*>(e_hi + row * e_ld + 4 * i) = *reinterpret_cast<const uint2*>(h);
+        if (e_lo) *reinterpret_cast<uint2*>(e_lo + row * e_ld + 4 * i) = *reinterpret_cast<const uint2*>(l);
+      }
     }
   }
 }
@@ -229,18 +240,26 @@ extern "C" int32_t b2a_coeffs_from_stats(const int64_t* stats, int32_t B, int32_
 
 extern "C" int32_t b2a_layernorm(const float* x, int64_t x_ld, const float* res, int64_t res_ld, float* y, int64_t y_ld,
                                  int64_t rows, int32_t C, const float* w, const float* b, const float* ada, float eps,
-                                 int32_t rms, int32_t post_act, float post_p0, void* stream) {
+                                 int32_t rms, int32_t post_act, float post_p0, void* emit_hi, void* emit_lo, int64_t emit_ld,
+                                 void* stream) {
   B2A_CHECK_ARG(x && y && rows >= 0 && C > 0, "bad pointers/shape");
   if (rows == 0) return B2A_OK;
   const bool al = C % 4 == 0 && C <= 1024 && x_ld % 4 == 0 && y_ld % 4 == 0 && (!res || res_ld % 4 == 0) && ((uintptr_t)x & 15) == 0 &&
                   ((uintptr_t)y & 15) == 0 && (!res || ((uintptr_t)res & 15) == 0);
+  B2A_CHECK_ARG(!emit_hi || (al && emit_ld >= C && emit_ld % 4 == 0 && ((uintptr_t)emit_hi & 7) == 0 && ((uintptr_t)emit_lo & 7) == 0),
+                "emitted planes need the vectorised kernel (C % 4 == 0, C <= 1024, 16-byte aligned rows), emit_ld >= C, a multiple of 4");
+  cudaStream_t st = (cudaStream_t)stream;
+  __nv_bfloat16 *eh = (__nv_bfloat16*)emit_hi, *el = (__nv_bfloat16*)emit_lo;
+  cudaError_t e = cudaSuccess;
   if (al && C <= 512)
-    layernorm_vec_kernel<4><<<cdiv(rows, 4), 128, 0, (cudaStream_t)stream>>>(x, x_ld, res, res_ld, y, y_ld, rows, C, w, b, ada, eps, rms, post_act, post_p0);
+    e = b2a_launch_pdl(layernorm_vec_kernel<4>, dim3(cdiv(rows, 4)), dim3(128), 0, st, x, x_ld, res, res_ld, y, y_ld, rows, (int)C, w, b,
+                       ada, eps, (int)rms, (int)post_act, post_p0, eh, el, emit_ld);
   else if (al)
-    layernorm_vec_kernel<8><<<cdiv(rows, 4), 128, 0, (cudaStream_t)stream>>>(x, x_ld, res, res_ld, y, y_ld, rows, C, w, b, ada, eps, rms, post_act, post_p0);
+    e = b2a_launch_pdl(layernorm_vec_kernel<8>, dim3(cdiv(rows, 4)), dim3(128), 0, st, x, x_ld, res, res_ld, y, y_ld, rows, (int)C, w, b,
+                       ada, eps, (int)rms, (int)post_act, post_p0, eh, el, emit_ld);
   else
-    layernorm_kernel<<<cdiv(rows, 8), 256, 0, (cudaStream_t)stream>>>(x, x_ld, res, res_ld, y, y_ld, rows, C, w, b, ada, eps,
-                                                                      rms, post_act, post_p0);
+    layernorm_kernel<<<cdiv(rows, 8), 256, 0, st>>>(x, x_ld, res, res_ld, y, y_ld, rows, C, w, b, ada, eps, rms, post_act, post_p0);
+  if (e != cudaSuccess) { b2a_set_error("b2a_layernorm: %s", cudaGetErrorString(e)); return B2A_E_CUDA; }
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }

@@ -11,6 +11,27 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// The hi / lo split of every tensor-core A operand: hi = 16-bit(v), lo = 16-bit(v - hi).  Producers that emit their consumer's planes
+// directly use this same helper as the prep kernels, so the planes are bit-identical whichever kernel writes them.
+template <typename T> __device__ __forceinline__ T to16(float v);
+template <> __device__ __forceinline__ __nv_bfloat16 to16<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half to16<__half>(float v) { return __float2half_rn(v); }
+__device__ __forceinline__ float from16(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float from16(__half v) { return __half2float(v); }
+template <typename T> __device__ __forceinline__ void split16(float v, T& hi, T& lo) { hi = to16<T>(v); lo = to16<T>(v - from16(hi)); }
+
+// Operand planes of b2a_attention_tc inside its workspace: fp16 hi / lo of Q (pre-scaled) and K, [B*H][T][64], and of V transposed,
+// [B*H][64][tkp] with the keys zero-padded to a multiple of 8.  The qkv GEMM's epilogue (b2a_conv1d_tc) writes this layout directly.
+struct AttnOperands { __half *qh, *ql, *kh, *kl, *vh, *vl; int64_t tkp; };
+__host__ __device__ inline AttnOperands attn_operands(void* ws, int64_t bh, int Tq, int Tk) {
+  AttnOperands a;
+  a.tkp = ((int64_t)Tk + 7) / 8 * 8;
+  a.qh = (__half*)(((uintptr_t)ws + 255) & ~(uintptr_t)255); a.ql = a.qh + bh * Tq * 64;
+  a.kh = a.ql + bh * Tq * 64; a.kl = a.kh + bh * Tk * 64;
+  a.vh = a.kl + bh * Tk * 64; a.vl = a.vh + bh * 64 * a.tkp;
+  return a;
+}
+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }

@@ -216,8 +216,9 @@ def conv1d(x: torch.Tensor, cw: ConvW, *, stride=1, dilation=1, pad_left=0, lout
     or (y, None) when the layer does not run on that path."""
     if isinstance(x, Planes):                      # operand already split by its producer (conv1d(..., emit=...)): tensor-core path only
         B, L, cin = x.shape
-        if cin != cw.cin or pre is not None or not _tc_eligible(cw, L, stride, transpose, pad_mode, dilation) or x.hi.shape[2] != cw.cin_pad:
-            raise ValueError("conv1d: a Planes operand needs a tensor-core-eligible layer with matching channels and no prologue")
+        if (cin != cw.cin or pre is not None or not _tc_eligible(cw, L, stride, transpose, pad_mode, dilation) or x.hi.shape[2] != cw.cin_pad
+                or x.hi.dtype != (torch.float16 if cw.f16 else torch.bfloat16)):
+            raise ValueError("conv1d: a Planes operand needs a tensor-core-eligible layer with matching channels, dtype and no prologue")
         if lout is None:
             lout = (L + 2 * pad_left - dilation * (cw.K - 1) - 1) // stride + 1
         return _conv1d_tc(x, cw, dilation, pad_left, lout, None, post_act, post_p0, cscale, res, res_div, out_scale, out, accumulate,
@@ -293,6 +294,12 @@ def emit_eligible(cw: "ConvW", x: torch.Tensor, lout: int, stride: int = 1, dila
             and (128 + (cw.K - 1) * dilation) * 128 * 4 <= 160 * 1024)
 
 
+def emit_tc_eligible(cw: "ConvW", L: int) -> bool:
+    """True when ``linear(x, cw, planes=True / qkv_heads=)`` can run: a tensor-core Linear at L rows whose Cout needs no pad
+    channels in its consumer's bf16 planes."""
+    return cw.K == 1 and not cw.f16 and cw.cout % 64 == 0 and _tc_eligible(cw, L, 1, False, 0)
+
+
 def prep_bf16(x: torch.Tensor, pre: Optional[Pre], cpad: int, planes: int = 2, f16: bool = False):
     """Conv prologue -> (hi, lo) bf16 (or fp16) planes [B, L, cpad] (lo None when planes == 1)."""
     _chk3(x, "prep_bf16 x")
@@ -311,8 +318,24 @@ def prep_bf16(x: torch.Tensor, pre: Optional[Pre], cpad: int, planes: int = 2, f
 TC_STATS = [os.environ.get("B2A_TC_STATS", "0") != "0"]
 
 
+def _new_planes(B: int, L: int, C: int, device) -> Planes:
+    """Uninitialised bf16 planes [B, L, C] for a producer to fill (lo only in "x2" mode)."""
+    return Planes(torch.empty(B, L, C, device=device, dtype=torch.bfloat16),
+                  torch.empty(B, L, C, device=device, dtype=torch.bfloat16) if TC_MODE[0] == "x2" else None, C)
+
+
+@dataclass
+class AttnPlanes:
+    """The q / k / v operands of the tensor-core attention, already split into its fp16 planes (q pre-scaled) inside its workspace
+    ``ws`` by the fused qkv projection's epilogue: ``linear(x, cw, qkv_heads=H, qkv_scale=s)``."""
+    ws: torch.Tensor
+    B: int
+    T: int
+    H: int
+
+
 def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, res, res_div, out_scale, out, accumulate,
-               up_stride=0, stats=False):
+               up_stride=0, stats=False, emit: Optional[Planes] = None, attn: Optional[AttnPlanes] = None, attn_scale=0.0):
     if isinstance(x, Planes):
         B, L, _ = x.shape
         hi, lo = x.hi, x.lo
@@ -344,7 +367,9 @@ def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, 
         ws = torch.empty(B, slots, cw.cout, 2, device=hi.device, dtype=torch.float64)
     _call("conv_tc", _lib.lib().b2a_conv1d_tc, 1, hi.data_ptr(), _p(lo), int(cw.f16), B, L, cw.cin_pad, w_tc.data_ptr(), _p(w_lo), taps, shifts, n_total, lout,
           _p(cw.bias), post_act, post_p0, cs, cs_bs, r, r_bs, r_ld, res_div, out_scale, int(accumulate), out.data_ptr(), out.stride(0),
-          out.stride(1), up_stride, pad_left if up_stride else 0, _p(ws), slots, _stream())
+          out.stride(1), up_stride, pad_left if up_stride else 0, _p(ws), slots,
+          None if emit is None else emit.hi.data_ptr(), None if emit is None else _p(emit.lo), 0 if emit is None else emit.hi.stride(1),
+          None if attn is None else attn.ws.data_ptr(), 0 if attn is None else attn.H, float(attn_scale), _stream())
     return (out, ws) if stats else out
 
 
@@ -517,9 +542,41 @@ def conv_fused(problems) -> list:
     return [pr.out for pr in problems]
 
 
-def linear(x: torch.Tensor, cw: ConvW, **kw) -> torch.Tensor:
-    """nn.Linear on [..., in] via the K=1 conv; accepts [rows, in] or [B, L, in]."""
-    if x.dim() == 2:
+def linear(x, cw: ConvW, *, planes=False, qkv_heads=0, qkv_scale=0.0, **kw):
+    """nn.Linear on [..., in] via the K=1 conv; accepts [rows, in] or [B, L, in], or the ``Planes`` a producer emitted.
+
+    ``planes=True`` returns (y, Planes): the epilogue also writes y's bf16 planes for the next GEMM.  ``qkv_heads=H`` returns
+    (y, AttnPlanes): y is a fused [q | k | v] projection and the epilogue writes the operands of ``attention_planes`` (``qkv_scale``
+    is the attention's softmax scale).  Both need the tensor-core path (``emit_tc_eligible``) and a 3-D operand."""
+    if planes or qkv_heads:
+        if isinstance(x, torch.Tensor) and x.dim() != 3:
+            raise ValueError("linear: planes= / qkv_heads= need a 3-D operand")
+        B, L, _ = x.shape
+        if not emit_tc_eligible(cw, L):
+            raise ValueError("linear: planes= / qkv_heads= need a tensor-core layer (ops.emit_tc_eligible)")
+        for k in ("out", "res"):
+            t = kw.get(k)
+            if t is not None and t.dim() == 2:
+                kw[k] = t[None]
+        out, pre, res = kw.pop("out", None), kw.pop("pre", None), kw.pop("res", None)
+        post_act, post_p0, cscale, out_scale = kw.pop("post_act", 0), kw.pop("post_p0", 0.0), kw.pop("cscale", None), kw.pop("out_scale", 1.0)
+        if kw:
+            raise TypeError(f"linear: unsupported arguments with planes= / qkv_heads=: {sorted(kw)}")
+        if isinstance(x, Planes) and (pre is not None or x.C != cw.cin or x.hi.shape[2] != cw.cin_pad or x.hi.dtype != torch.bfloat16):
+            raise ValueError("linear: a Planes operand needs matching channels and dtype and takes no prologue")
+        if out is None:
+            out = torch.empty(B, L, cw.cout, device=cw.w.device, dtype=torch.float32)
+        em = at = None
+        if qkv_heads:
+            if cw.cout != 3 * 64 * qkv_heads:
+                raise ValueError(f"linear: qkv_heads={qkv_heads} needs Cout = {3 * 64 * qkv_heads}, got {cw.cout}")
+            at = AttnPlanes(torch.empty(_lib.lib().b2a_attention_tc_ws_bytes(B, qkv_heads, L, L), device=out.device, dtype=torch.uint8),
+                            B, L, qkv_heads)
+        else:
+            em = _new_planes(B, L, cw.cout, out.device)
+        y = _conv1d_tc(x, cw, 1, 0, L, pre, post_act, post_p0, cscale, res, 1, out_scale, out, False, emit=em, attn=at, attn_scale=qkv_scale)
+        return y, (at if qkv_heads else em)
+    if isinstance(x, torch.Tensor) and x.dim() == 2:
         o = kw.get("out")
         if o is not None and o.dim() == 2:
             kw["out"] = o[None]
@@ -632,8 +689,9 @@ def coeffs_from_stats(stats: torch.Tensor, L: int, gb: Optional[torch.Tensor], e
 
 
 def layernorm(x: torch.Tensor, w=None, b=None, *, eps=1e-5, res=None, ada=None, rms=False, post_act=0, post_p0=0.0,
-              out=None) -> torch.Tensor:
-    """Row LayerNorm / RMSNorm over the last dim of a 2-D row-strided view."""
+              out=None, planes=False):
+    """Row LayerNorm / RMSNorm over the last dim of a 2-D row-strided view.  ``planes=True`` returns (y, Planes [1, rows, C]): the
+    kernel also writes y's bf16 planes for the next GEMM (C a multiple of 64, so that they need no pad channels)."""
     shp = x.shape
     x2 = x.reshape(-1, shp[-1]) if x.dim() != 2 else x
     assert x2.stride(1) == 1
@@ -643,10 +701,17 @@ def layernorm(x: torch.Tensor, w=None, b=None, *, eps=1e-5, res=None, ada=None, 
     if out is None:
         out = torch.empty(x2.shape, device=x.device, dtype=torch.float32)
     o2 = out.reshape(-1, shp[-1]) if out.dim() != 2 else out
+    pl = None
+    if planes:
+        if shp[-1] % 64:
+            raise ValueError(f"layernorm: planes=True needs C % 64 == 0, got {shp[-1]}")
+        pl = _new_planes(1, x2.shape[0], shp[-1], x.device)
     _call("layernorm", _lib.lib().b2a_layernorm, 1, x2.data_ptr(), x2.stride(0), _p(r2), 0 if r2 is None else r2.stride(0), o2.data_ptr(),
                                         o2.stride(0), x2.shape[0], shp[-1], _p(w), _p(b), _p(ada), eps, int(rms), post_act,
-                                        post_p0, _stream())
-    return out.reshape(shp) if out.dim() == 2 and len(shp) != 2 else out
+                                        post_p0, None if pl is None else pl.hi.data_ptr(), None if pl is None else _p(pl.lo),
+                                        shp[-1], _stream())
+    y = out.reshape(shp) if out.dim() == 2 and len(shp) != 2 else out
+    return (y, pl) if planes else y
 
 
 def attention(q, k, v, *, n_heads, n_kv_heads=None, scale, causal=False, q_offset=0, window=0, k_len=None, out=None):
@@ -672,6 +737,26 @@ def attention(q, k, v, *, n_heads, n_kv_heads=None, scale, causal=False, q_offse
         return out
     _call("attention", _lib.lib().b2a_attention, 1, C.byref(p), _stream())
     return out
+
+
+def attention_planes(ap: AttnPlanes, *, planes=False, out=None):
+    """Non-causal tensor-core attention over the operands a fused qkv projection emitted (``linear(..., qkv_heads=)``): one launch.
+    Returns ctx [B, T, H*64], or (ctx, Planes) with ``planes=True`` (ctx's bf16 planes for the output projection)."""
+    B, T, H = ap.B, ap.T, ap.H
+    if T < 64:
+        raise ValueError("attention_planes: the tensor-core attention needs at least 64 keys")
+    if out is None:
+        out = torch.empty(B, T, H * 64, device=ap.ws.device, dtype=torch.float32)
+    _chk3(out, "attention_planes out")
+    pl = _new_planes(B, T, H * 64, out.device) if planes else None
+    p = AttnParams()
+    p.o, p.o_bs, p.o_ld = out.data_ptr(), out.stride(0), out.stride(1)
+    p.B, p.Tq, p.Tk, p.H, p.Hkv, p.D = B, T, T, H, H, 64
+    p.operands_ready = 1
+    if pl is not None:
+        p.emit_hi, p.emit_lo, p.emit_ld = pl.hi.data_ptr(), _p(pl.lo), H * 64
+    _call("attention", _lib.lib().b2a_attention_tc, 1, C.byref(p), ap.ws.data_ptr(), _stream())
+    return (out, pl) if planes else out
 
 
 def rope_(x: torch.Tensor, n_heads: int, *, offset=0, base=10000.0, traditional=True) -> torch.Tensor:

@@ -555,18 +555,34 @@ class Model:
                 text_branch()
         # ---- ALBERT
         e = ops.gather_rows(W["word_emb"], ids)
-        e = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T])
-        h = ops.linear(e, W["map_in"])
         nh = cfg.plbert["num_attention_heads"]
         hs = cfg.plbert["hidden_size"]
-        for _ in range(cfg.plbert["num_hidden_layers"]):
-            qkv = ops.linear(h, W["qkv"])[None]                       # [1,T,3*hs]
-            ctx = ops.attention(qkv[:, :, :hs], qkv[:, :, hs:2 * hs], qkv[:, :, 2 * hs:], n_heads=nh, scale=1.0 / math.sqrt(hs // nh))[0]
-            a = ops.linear(ctx, W["attn_out"], res=h)
-            a = ops.layernorm(a, *W["attn_ln"], eps=1e-12)
-            f1 = ops.linear(a, W["ffn"], post_act=ACT["gelu"])
-            f2 = ops.linear(f1, W["ffn_out"], res=a)
-            h = ops.layernorm(f2, *W["full_ln"], eps=1e-12)
+        scale = 1.0 / math.sqrt(hs // nh)
+        if self._albert_planes(T):
+            # 7 launches per layer: every producer also writes its consumer's 16-bit operand planes (no prep kernels), the qkv
+            # projection those of the attention; bit-identical to the branch below
+            _, ep = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T], planes=True)
+            h, hp = ops.linear(ep, W["map_in"], planes=True)
+            for _ in range(cfg.plbert["num_hidden_layers"]):
+                _, qkv = ops.linear(hp, W["qkv"], qkv_heads=nh, qkv_scale=scale)
+                _, cp = ops.attention_planes(qkv, planes=True)
+                a = ops.linear(cp, W["attn_out"], res=h)
+                a, ap = ops.layernorm(a, *W["attn_ln"], eps=1e-12, planes=True)
+                _, fp = ops.linear(ap, W["ffn"], post_act=ACT["gelu"], planes=True)
+                f2 = ops.linear(fp, W["ffn_out"], res=a)
+                h, hp = ops.layernorm(f2, *W["full_ln"], eps=1e-12, planes=True)
+            h = h[0]
+        else:
+            e = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T])
+            h = ops.linear(e, W["map_in"])
+            for _ in range(cfg.plbert["num_hidden_layers"]):
+                qkv = ops.linear(h, W["qkv"])[None]                       # [1,T,3*hs]
+                ctx = ops.attention(qkv[:, :, :hs], qkv[:, :, hs:2 * hs], qkv[:, :, 2 * hs:], n_heads=nh, scale=scale)[0]
+                a = ops.linear(ctx, W["attn_out"], res=h)
+                a = ops.layernorm(a, *W["attn_ln"], eps=1e-12)
+                f1 = ops.linear(a, W["ffn"], post_act=ACT["gelu"])
+                f2 = ops.linear(f1, W["ffn_out"], res=a)
+                h = ops.layernorm(f2, *W["full_ln"], eps=1e-12)
         self._tap("bert", h)
         # ---- duration encoder: X640 = [d_en | style]
         stl = cfg.style_dim
@@ -593,6 +609,14 @@ class Model:
         self._tap("t_en", t_en)
         st.update(X=X, t_en=t_en, pred=pred, idx=idx, total=total)
         return st
+
+    def _albert_planes(self, T: int) -> bool:
+        """ALBERT runs as the plane-emitting launch chain when every GEMM takes the tensor-core path at T rows and the attention the
+        tensor-core kernel (64-wide heads, at least 64 keys); otherwise (short utterances, B2A_TC=off, B2A_ATTN=cuda) as separate ops."""
+        W, pb = self._w, self.config.plbert
+        return (T >= 64 and ops.ATTN_MODE[0] == "tc" and pb["hidden_size"] == 64 * pb["num_attention_heads"]
+                and pb["hidden_size"] % 64 == 0 and W["map_in"].cin % 64 == 0
+                and all(ops.emit_tc_eligible(W[k], T) for k in ("map_in", "qkv", "attn_out", "ffn", "ffn_out")))
 
     def _bind(self, st):
         """Point the style-projection lookups (`_gb`) at this utterance's rows."""
