@@ -114,6 +114,10 @@ int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16, int32_t B
  * (entry, setup done, first operands landed, last operands landed, accumulator ready, epilogue done, exit); NULL disables. */
 int32_t b2a_conv1d_tc_debug(void* dbg8);
 
+/* tiling of the calling host thread's last successful b2a_conv1d_tc launch: out[0..4] = N tile (BN), grid x (row tiles), grid y
+ * (Cout / BN), grid z (batch), operand stages; all zero before the first launch.  Host-side record only. */
+int32_t b2a_conv1d_tc_last_config(int32_t* out5);
+
 /* strided 2-D copy (concat without torch.cat): dst[r, c] = src[r, c] */
 int32_t b2a_copy2d(const float* src, int64_t src_ld, float* dst, int64_t dst_ld, int64_t rows, int32_t cols, void* stream);
 /* dst[r, :] = src[idx[r], :] (+ add[r % add_period, :] if add != NULL) -- the alignment expansion `x @ pred_aln_trg` of
@@ -253,6 +257,9 @@ typedef struct {
 } b2a_convf_t;
 int32_t b2a_conv1d_fused_debug(void* stamps /* device uint64 [grid][16] or NULL: phase time stamps of the next launches */);
 int32_t b2a_conv1d_fused(const b2a_convf_t* problems, int32_t n_problems, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream);
+/* tiling of the calling host thread's last successful b2a_conv1d_fused launch: out[0] = problems, out[1] = grid (CTAs),
+ * out[2 + 2 i], out[3 + 2 i] = N tile and K split of problem i in the caller's order (i < 4, unused slots zero).  Host-side only. */
+int32_t b2a_conv1d_fused_last_config(int32_t* out10);
 
 /* out[i] ~ N(0,1), i < n: Philox4x32-10 keyed by `seed`, counter `offset + i/4`, Box-Muller.  The production replacement for
  * mx.random.normal in SineGen / NoiseBlock (istftnet.py:649, snac/layers.py:263); parity tests inject the noise instead. */

@@ -705,6 +705,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_enc = nullptr;
 unsigned long long* g_fdbg = nullptr;
+thread_local int32_t g_last_cfg[2 + 2 * MAXG] = {};    // problems, grid, then (BN, ksplit) per problem: this host thread's last launch
 
 int get_enc() {
   if (g_enc) return 0;
@@ -729,6 +730,13 @@ int make_wmap(CUtensorMap* m, const void* base, uint64_t cin_pad, uint64_t rows,
 
 /* debug aid: device buffer of [gridDim][32] uint64 that the next launches stamp with %globaltimer at their phase boundaries (NULL: off) */
 extern "C" int32_t b2a_conv1d_fused_debug(void* buf) { g_fdbg = (unsigned long long*)buf; return B2A_OK; }
+
+/* the tiles and K splits the last launch chose, so that tests can assert which variant they exercised */
+extern "C" int32_t b2a_conv1d_fused_last_config(int32_t* out10) {
+  B2A_CHECK_ARG(out10, "null pointer");
+  for (int i = 0; i < 2 + 2 * MAXG; i++) out10[i] = g_last_cfg[i];
+  return B2A_OK;
+}
 
 extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream) {
   B2A_CHECK_ARG(pr && n >= 1 && n <= MAXG && (planes == 1 || planes == 2), "1..4 problems, planes 1 or 2");
@@ -873,5 +881,8 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
                         : cudaLaunchKernelEx(&cfg, conv_fused_kernel<false>, p, mw[0], mw[1], mw[2], mw[3], ml[0], ml[1], ml[2], ml[3]);
   if (err != cudaSuccess) { b2a_set_error("b2a_conv1d_fused: launch failed: %s", cudaGetErrorString(err)); return B2A_E_CUDA; }
   B2A_CHECK_LAUNCH();
+  for (int i = 0; i < 2 + 2 * MAXG; i++) g_last_cfg[i] = 0;
+  g_last_cfg[0] = n; g_last_cfg[1] = grid;
+  for (int gi = 0; gi < n; gi++) { g_last_cfg[2 + 2 * order[gi]] = p.pr[gi].BN; g_last_cfg[3 + 2 * order[gi]] = p.pr[gi].ksplit; }
   return B2A_OK;
 }

@@ -339,6 +339,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode = nullptr;
 long long* g_dbg = nullptr;
+thread_local int32_t g_last_cfg[5] = {0, 0, 0, 0, 0};   // BN, grid x / y / z, stages of this host thread's last launch
 
 int get_encode() {
   if (g_encode) return 0;
@@ -363,6 +364,13 @@ int make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, c
 
 /* debug aid: device buffer of 8 int64 that the next b2a_conv1d_tc launches stamp with clock64() at their phase boundaries */
 extern "C" int32_t b2a_conv1d_tc_debug(void* dbg8) { g_dbg = (long long*)dbg8; return B2A_OK; }
+
+/* the tile the dispatch rule chose for the last launch, so that tests can assert which kernel variant they exercised */
+extern "C" int32_t b2a_conv1d_tc_last_config(int32_t* out5) {
+  B2A_CHECK_ARG(out5, "null pointer");
+  for (int i = 0; i < 5; i++) out5[i] = g_last_cfg[i];
+  return B2A_OK;
+}
 
 extern "C" int32_t b2a_prep_bf16(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t C, int32_t cpad,
                                  const float* scale, const float* shift, int32_t act, float p0, const float* a, const float* b,
@@ -480,5 +488,6 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
     b2a_set_error("b2a_conv1d_tc: %s", cudaGetErrorString(cudaGetLastError()));
     return B2A_E_CUDA;
   }
+  g_last_cfg[0] = p.BN; g_last_cfg[1] = (int32_t)grid.x; g_last_cfg[2] = (int32_t)grid.y; g_last_cfg[3] = (int32_t)grid.z; g_last_cfg[4] = p.stages;
   return B2A_OK;
 }

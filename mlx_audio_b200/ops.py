@@ -373,6 +373,21 @@ def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, 
     return (out, ws) if stats else out
 
 
+def conv1d_tc_last_config() -> dict:
+    """Tiling of this host thread's last b2a_conv1d_tc launch: {"BN", "grid": (x, y, z), "stages"} (BN 0 before any launch)."""
+    out = (C.c_int32 * 5)()
+    _lib.check(_lib.lib().b2a_conv1d_tc_last_config(out))
+    return {"BN": out[0], "grid": (out[1], out[2], out[3]), "stages": out[4]}
+
+
+def conv1d_fused_last_config() -> dict:
+    """Tiling of this host thread's last b2a_conv1d_fused launch: {"grid", "BN": [per problem], "ksplit": [per problem]}, problems in
+    the order they were passed."""
+    out = (C.c_int32 * 10)()
+    _lib.check(_lib.lib().b2a_conv1d_fused_last_config(out))
+    n = out[0]
+    return {"grid": out[1], "BN": [out[2 + 2 * i] for i in range(n)], "ksplit": [out[3 + 2 * i] for i in range(n)]}
+
 
 # ---------------------------------------------------------------------------------------------------------------- fused wgmma conv
 # One launch per layer (or per GROUP of independent layers): InstanceNorm / AdaIN coefficients from the producer's (sum, sumsq), the

@@ -573,16 +573,19 @@ class Model:
                 h, hp = ops.layernorm(f2, *W["full_ln"], eps=1e-12, planes=True)
             h = h[0]
         else:
-            e = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T])
-            h = ops.linear(e, W["map_in"])
-            for _ in range(cfg.plbert["num_hidden_layers"]):
-                qkv = ops.linear(h, W["qkv"])[None]                       # [1,T,3*hs]
-                ctx = ops.attention(qkv[:, :, :hs], qkv[:, :, hs:2 * hs], qkv[:, :, 2 * hs:], n_heads=nh, scale=scale)[0]
-                a = ops.linear(ctx, W["attn_out"], res=h)
-                a = ops.layernorm(a, *W["attn_ln"], eps=1e-12)
-                f1 = ops.linear(a, W["ffn"], post_act=ACT["gelu"])
-                f2 = ops.linear(f1, W["ffn_out"], res=a)
-                h = ops.layernorm(f2, *W["full_ln"], eps=1e-12)
+            # The GEMMs stay on conv_tc like the chain's: above 256 rows the fused kernel would take them and split K across CTAs,
+            # which sums in a different order.
+            with ops.fused_dispatch(False):
+                e = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T])
+                h = ops.linear(e, W["map_in"])
+                for _ in range(cfg.plbert["num_hidden_layers"]):
+                    qkv = ops.linear(h, W["qkv"])[None]                       # [1,T,3*hs]
+                    ctx = ops.attention(qkv[:, :, :hs], qkv[:, :, hs:2 * hs], qkv[:, :, 2 * hs:], n_heads=nh, scale=scale)[0]
+                    a = ops.linear(ctx, W["attn_out"], res=h)
+                    a = ops.layernorm(a, *W["attn_ln"], eps=1e-12)
+                    f1 = ops.linear(a, W["ffn"], post_act=ACT["gelu"])
+                    f2 = ops.linear(f1, W["ffn_out"], res=a)
+                    h = ops.layernorm(f2, *W["full_ln"], eps=1e-12)
         self._tap("bert", h)
         # ---- duration encoder: X640 = [d_en | style]
         stl = cfg.style_dim

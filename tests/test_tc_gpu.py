@@ -39,8 +39,8 @@ CASES = [
     (1, 129, 96, 32, 5, 2, 4),
     (1, 5000, 128, 128, 3, 1, 1),
     (1, 3000, 64, 64, 1, 1, 0),
-    (2, 700, 96, 96, 7, 9, 54),          # Qwen3 vocoder block 4: N tile 96, taps spanning 54 rows
-    (1, 40000, 192, 192, 7, 3, 18),      # N tile 96, several waves of CTAs
+    (2, 700, 96, 96, 7, 9, 54),          # Qwen3 vocoder block 4, taps spanning 54 rows; 12 row tiles: 32-wide N tiles on conv_tc
+    (1, 40000, 192, 192, 7, 3, 18),      # 96-wide N tiles, several waves of CTAs (every N tile: test_gemm_tc_matrix_gpu.py)
     (1, 600, 384, 384, 1, 1, 0),
     (1, 5000, 32, 64, 1, 1, 0),          # Mimi's last residual 1x1 (hidden 32): half of the 64-wide K chunk is zero padding
 ]
