@@ -366,6 +366,26 @@ int32_t b2a_snac_from_codes(const int64_t* const* codes_host_ptrs, const int32_t
                             const float* const* emb_host_ptrs, const float* const* w_host_ptrs, const float* const* bias_host_ptrs,
                             int32_t B, int64_t T, int32_t bins, int32_t cd, int32_t dim, float* out, int32_t* err_flag_dev, void* stream);
 
+/* ---- streaming decoder state (stream.cu) ------------------------------------------------------
+ * One entry of a grouped row-range launch on fp32 [B, rows, C] views: dst[b, r, c] = src[b, r, c] (COPY) or += (ADD), element
+ * (b, r, c) at b * bs + r * ld + c.  The incremental Qwen3-TTS speech-tokenizer decoder keeps its state with it:
+ *   COPY: the last (K-1)*dilation input rows of a causal conv become the history head of the next call's input buffer -- replaces
+ *         CausalConv1d.step (speech_tokenizer.py:71-83), ConvNeXtBlock.step's depthwise conv (:151-159), DecoderInitialConv.step
+ *         (:719-728) and DecoderOutputConv.step (:771-780); also the KV-cache growth of the decoder transformer (:610-617);
+ *   ADD:  the r-row overflow of a decoder block's transposed conv (bias included) is added into the head rows of the next call's
+ *         output -- DecoderBlockUpsample.step (:645-656). */
+#define B2A_ROWOP_COPY 0
+#define B2A_ROWOP_ADD 1
+#define B2A_ROWOPS_MAX 32
+typedef struct {
+  const float* src; int64_t src_bs, src_ld;
+  float* dst; int64_t dst_bs, dst_ld;
+  int32_t B, rows, C, op;
+} b2a_rowop_t;
+/* All n <= B2A_ROWOPS_MAX entries in one launch.  Entries run concurrently: an entry's destination may not overlap its own source or
+ * any range another entry reads or writes (B2A_E_INVALID otherwise).  Empty entries are skipped. */
+int32_t b2a_stream_rows(const b2a_rowop_t* ops, int32_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

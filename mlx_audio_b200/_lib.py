@@ -61,6 +61,15 @@ class ConvFParams(C.Structure):
     ]
 
 
+class RowOp(C.Structure):
+    """Mirror of b2a_rowop_t."""
+    _fields_ = [("src", C.c_void_p), ("src_bs", i64), ("src_ld", i64), ("dst", C.c_void_p), ("dst_bs", i64), ("dst_ld", i64),
+                ("B", i32), ("rows", i32), ("C", i32), ("op", i32)]
+
+
+ROWOPS_MAX = 32      # B2A_ROWOPS_MAX
+
+
 # name -> (restype, argtypes); every symbol include/b200audio.h declares
 PROTOTYPES = {
     "b2a_last_error": (C.c_char_p, []),
@@ -113,6 +122,7 @@ PROTOTYPES = {
     "b2a_rvq_encode": (i32, [c_f, i64, i64, i32, c_f, c_f, i32, i32, i32, c_f, i64, i64, C.c_void_p]),
     "b2a_snac_from_codes": (i32, [C.POINTER(C.c_void_p), C.POINTER(i32), i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                   C.POINTER(C.c_void_p), i32, i64, i32, i32, i32, c_f, c_f, C.c_void_p]),
+    "b2a_stream_rows": (i32, [C.POINTER(RowOp), i32, C.c_void_p]),
 }
 
 E_INVALID, E_CUDA, E_UNSUPPORTED = -1, -2, -3

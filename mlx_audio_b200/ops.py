@@ -609,6 +609,25 @@ def copy2d(src: torch.Tensor, dst: torch.Tensor) -> None:
     _call("other", _lib.lib().b2a_copy2d, 1, src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), rows, cols, _stream())
 
 
+def stream_rows(entries) -> None:
+    """One grouped launch of row-range moves: ``entries`` = [(src, dst, add)], src / dst float32 [B, rows, C] views of equal shape
+    (row-strided), dst = src (``add`` False) or dst += src.  No entry may write rows another entry reads or writes (the C side checks)."""
+    entries = [e for e in entries if e[0].numel()]
+    if len(entries) > _lib.ROWOPS_MAX:
+        raise ValueError(f"stream_rows: at most {_lib.ROWOPS_MAX} entries per launch, got {len(entries)}")
+    if not entries:
+        return
+    arr = (_lib.RowOp * len(entries))()
+    for i, (src, dst, add) in enumerate(entries):
+        _chk3(src, "stream_rows src")
+        _chk3(dst, "stream_rows dst")
+        if src.shape != dst.shape:
+            raise ValueError(f"stream_rows: source {tuple(src.shape)} and destination {tuple(dst.shape)} differ")
+        B, rows, Cc = src.shape
+        arr[i] = _lib.RowOp(src.data_ptr(), src.stride(0), src.stride(1), dst.data_ptr(), dst.stride(0), dst.stride(1), B, rows, Cc, int(bool(add)))
+    _call("other", _lib.lib().b2a_stream_rows, 1, arr, len(entries), _stream())
+
+
 def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor] = None, add: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[r, :] = src[idx[r], :] (+ add[r % add.shape[0], :]); src [N, C] float32, idx int64 [R]."""
     assert src.dim() == 2 and src.stride(1) == 1 and idx.dtype == torch.int64 and idx.is_contiguous()
@@ -1016,14 +1035,17 @@ def incr_(p: torch.Tensor, v: int = 1) -> None:
     _call("other", _lib.lib().b2a_incr_i32, 1, p.data_ptr(), v, _stream())
 
 
-def rvq_decode(codes: torch.Tensor, codebooks: torch.Tensor, out: Optional[torch.Tensor] = None, check=True) -> torch.Tensor:
-    """codes int64 [B,nq,T], codebooks [nq,bins,dim] -> sum of gathers [B,T,dim]."""
-    assert codes.dtype == torch.int64 and codes.stride(2) == 1 and codebooks.is_contiguous()
+def rvq_decode(codes: torch.Tensor, codebooks: torch.Tensor, out: Optional[torch.Tensor] = None, check=True,
+               err: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """codes int64 [B,nq,T], codebooks [nq,bins,dim] -> sum of gathers [B,T,dim].  ``err``: a zeroed int32 [1] flag to reuse (saves
+    the fill kernel of a fresh one); it stays zero unless a code is out of range."""
+    assert codes.dtype == torch.int64 and (codes.stride(2) == 1 or codes.shape[2] == 1) and codebooks.is_contiguous()
     B, nq, T = codes.shape
     _, bins, dim = codebooks.shape
     if out is None:
         out = torch.empty(B, T, dim, device=codes.device, dtype=torch.float32)
-    err = torch.zeros(1, device=codes.device, dtype=torch.int32)
+    if err is None:
+        err = torch.zeros(1, device=codes.device, dtype=torch.int32)
     _call("rvq", _lib.lib().b2a_rvq_decode, 1, codes.data_ptr(), codes.stride(0), codes.stride(1), B, nq, T, codebooks.data_ptr(), bins,
                                          dim, out.data_ptr(), out.stride(1), err.data_ptr(), _stream())
     if check and int(err.item()) != 0:

@@ -243,10 +243,7 @@ class Model:
         return self._rng
 
     @torch.no_grad()
-    def generate_codes(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, max_tokens: int = 4096, temperature: float = 0.9,
-                       top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, u=None, seed: int = 0,
-                       use_graph: bool = True, stop_on_eos: bool = True, left_padding=None, batch_mode: bool = False,
-                       trailing_rule: str = "clamp_pad"):
+    def generate_codes(self, input_embeds, trailing_text_hidden, tts_pad_embed, **kw):
         """The generation loop of Model.generate for B prompts of equal prefill length: returns int64 codes [B, n_frames, 16]
         (B = 1: frames up to, not including, EOS; B > 1: until every row has hit EOS, rows padded with code 0 after their EOS,
         the convention of batch_generate / batch_decode).  ``u`` [max_tokens, 16, B] uniforms in [0,1) (drawn from ``seed`` when
@@ -258,6 +255,20 @@ class Model:
         lengths [B]) with rows zero-padded after their EOS.  ``trailing_rule="standard"`` is the rule of the default (non-streaming)
         batch path, where every row behaves as a single sequence (continuous_batching.py:261-278: text while its index is inside the
         trailing text, pad afterwards): one extra pad row is appended so that the kernel's clamp lands on it."""
+        frames = self._frame_iter(input_embeds, trailing_text_hidden, tts_pad_embed, **kw)
+        while True:
+            try:
+                next(frames)
+            except StopIteration as stop:
+                return stop.value
+
+    @torch.no_grad()
+    def _frame_iter(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, max_tokens: int = 4096, temperature: float = 0.9,
+                    top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, u=None, seed: int = 0,
+                    use_graph: bool = True, stop_on_eos: bool = True, left_padding=None, batch_mode: bool = False,
+                    trailing_rule: str = "clamp_pad"):
+        """The loop of ``generate_codes`` as a generator: outside batch mode it yields (out, n) after every recorded frame -- ``out``
+        [B, max_tokens, 16] is the device buffer whose first n frames are final -- and returns what ``generate_codes`` returns."""
         t, cfg, dev = self.talker, self.config.talker_config, self.device
         x = input_embeds.to(dev).float().contiguous()
         B, P, H = x.shape
@@ -348,6 +359,7 @@ class Model:
             else:
                 out[:, n] = self._codes
             n += 1
+            yield out, n
         if int(self._err.item()) != 0:
             raise ValueError("generate_codes: a sampled code indexed outside its embedding table")
         self._graph = graph
@@ -444,13 +456,55 @@ class Model:
             audio = audio[:valid]
         return audio
 
+    def _stream_segment(self, x, trailing, pad, segment_idx: int, streaming_interval: float, gen: dict):
+        """The streaming branch of the generation loop (qwen3_tts.py:1316-1521, 2264-2446): after every recorded frame, once
+        ``max(1, int(streaming_interval * 12.5))`` frames are undecoded, decode them with the incremental decoder and yield a chunk;
+        after EOS / ``max_tokens`` yield the rest (if any) as the final chunk.  Streamed audio is not trimmed to the valid length."""
+        dec = self.speech_tokenizer.decoder
+        chunk = max(1, int(streaming_interval * 12.5))
+        dec.reset_streaming_state()
+        t0 = time.perf_counter()
+
+        def event(codes, n_new, n_total, final):
+            nonlocal t0
+            audio = dec.streaming_step(codes.transpose(1, 2))[0, 0]
+            torch.cuda.synchronize(self.device)
+            dt = time.perf_counter() - t0
+            samples = int(audio.shape[0])
+            dur = samples / self.sample_rate
+            audio_samples = {"samples": samples, "samples-per-sec": samples / dt if dt > 0 else 0}
+            if not final:
+                audio_samples["tokens"] = n_total
+            res = GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=segment_idx, token_count=n_new,
+                                   audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0,
+                                   prompt={"tokens": n_new, "tokens-per-sec": n_new / dt if dt > 0 else 0}, audio_samples=audio_samples,
+                                   processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9,
+                                   is_streaming_chunk=True, is_final_chunk=final)
+            t0 = time.perf_counter()
+            return res
+
+        decoded, out, n = 0, None, 0
+        for out, n in self._frame_iter(x, trailing, pad, **gen):
+            if n - decoded >= chunk:
+                yield event(out[:1, decoded:n], n - decoded, n, False)
+                decoded = n
+        if n > decoded:
+            yield event(out[:1, decoded:n], n - decoded, n, True)
+        dec.reset_streaming_state()
+
     def generate_from_ids(self, input_ids, *, language_id=None, speaker_id=None, temperature: float = 0.9, max_tokens: int = 4096,
-                          top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, seed: int = 0, u=None, **kwargs):
-        """``Model.generate`` (qwen3_tts.py:1122-1575) for one already-tokenised segment; yields one GenerationResult."""
+                          top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, seed: int = 0, u=None,
+                          stream: bool = False, streaming_interval: float = 2.0, **kwargs):
+        """``Model.generate`` (qwen3_tts.py:1122-1575) for one already-tokenised segment; yields one GenerationResult, or with
+        ``stream=True`` one per ``streaming_interval`` seconds of generated frames (the last with ``is_final_chunk``)."""
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
         x, trailing, pad = self.prepare_generation_inputs_from_ids(input_ids, language_id, speaker_id)
+        if stream:
+            yield from self._stream_segment(x, trailing, pad, 0, streaming_interval, dict(
+                max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u))
+            return
         codes = self.generate_codes(x, trailing, pad, max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
                                     repetition_penalty=repetition_penalty, seed=seed, u=u)
         if codes.shape[1] == 0:
@@ -466,7 +520,7 @@ class Model:
                                audio_samples={"samples": samples, "samples-per-sec": round(samples / dt, 2) if dt > 0 else 0},
                                processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
 
-    def _generate_segments(self, text, split_pattern, speaker, language, instruct, **gen):
+    def _generate_segments(self, text, split_pattern, speaker, language, instruct, stream=False, streaming_interval=2.0, **gen):
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         # base path: segments are split AND stripped (qwen3_tts.py:1268-1271); the instruct paths pass split_pattern=None and the text as is
@@ -477,6 +531,9 @@ class Model:
             seg_gen = dict(gen)
             if seg_gen.get("seed") is not None:                       # a fixed seed still gives every segment its own draws
                 seg_gen["seed"] = int(seg_gen["seed"]) + idx
+            if stream:                                                # the instruct paths report segment 0 (qwen3_tts.py:2264-2446)
+                yield from self._stream_segment(x, trailing, pad, idx if split_pattern else 0, streaming_interval, seg_gen)
+                continue
             codes = self.generate_codes(x, trailing, pad, **seg_gen)
             if codes.shape[1] == 0:
                 continue
@@ -502,14 +559,14 @@ class Model:
             if not instruct:
                 raise ValueError("VoiceDesign model requires 'instruct' to describe the voice "
                                  "(e.g., 'A cheerful young female voice with high pitch')")
-            yield from self._generate_segments(text, None, None, lang_code, instruct, **gen)        # one utterance: _generate_with_instruct does not split
+            yield from self._generate_segments(text, None, None, lang_code, instruct, stream, streaming_interval, **gen)   # one utterance: no split
             return
         if kind == "custom_voice":
             if not voice:
                 raise ValueError(f"CustomVoice model requires 'voice' (speaker name) (e.g., {self.supported_speakers})")
             if voice.lower() not in [s.lower() for s in self.supported_speakers]:
                 raise ValueError(f"Speaker '{voice}' not supported. Available: {self.supported_speakers}")
-            yield from self._generate_segments(text, None, voice, lang_code, instruct, **gen)
+            yield from self._generate_segments(text, None, voice, lang_code, instruct, stream, streaming_interval, **gen)
             return
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
@@ -518,10 +575,7 @@ class Model:
             # Neither encoder has a CUDA path yet -- refuse instead of silently synthesising the default voice.
             raise NotImplementedError("voice cloning from ref_audio needs the speech-tokenizer encoder + speaker encoder "
                                       "(SURVEY.md section 8f 'next'); call without ref_audio for the default voice")
-        if stream:
-            raise NotImplementedError("stream=True (incremental audio chunks) is not implemented for generate(); use "
-                                      "batch_generate(stream=True) or speech_tokenizer.streaming_decode on the returned codes")
         if voice is not None and voice.lower() not in [s.lower() for s in self.supported_speakers]:
             raise ValueError(f"Voice '{voice}' is not supported by this Base model. Base models have no built-in preset voices — "
                              "clone a voice by passing ref_audio and ref_text instead.")
-        yield from self._generate_segments(text, split_pattern, voice, lang_code, None, **gen)
+        yield from self._generate_segments(text, split_pattern, voice, lang_code, None, stream, streaming_interval, **gen)

@@ -2,7 +2,7 @@
 
 ``Qwen3TTSSpeechTokenizer(cfg).load_weights(...)``; ``decode(audio_codes[B,T,16]) -> (wav[B,samples], lengths)``
 (speech_tokenizer.py:1099-1118), ``batch_decode`` (:1120-1179), ``streaming_decode`` (:1181-1217) and the decoder's
-``__call__`` / ``chunked_decode`` (:843-880, 932-954).
+``__call__`` / ``chunked_decode`` (:843-880, 932-954) and the incremental ``streaming_step`` / ``reset_streaming_state`` (:882-930).
 
 H100 mapping: RVQ gather-sum in one kernel; every dense conv / linear runs on the wgmma conv kernel with the SnakeBeta /
 LayerScale / gamma / residual / clip fused as prologue or epilogue; the 300-frame chunks of ``chunked_decode`` are
@@ -39,6 +39,7 @@ class Qwen3TTSSpeechTokenizerDecoder:
         self.device = torch.device(device)
         self.total_upsample = int(np.prod(list(config.upsample_rates) + list(config.upsampling_ratios)))
         self._w = None
+        self._st = None                 # streaming state (streaming_step); None = no stream in progress
 
     # ------------------------------------------------------------------ weights
     def load_weights(self, weights, prefix="decoder."):
@@ -169,10 +170,157 @@ class Qwen3TTSSpeechTokenizerDecoder:
                 out[:, :, s * up: e * up] = wav[i * B: (i + 1) * B, :, c * up:]
         return out
 
-    # streaming (speech_tokenizer.py:882-930) re-decodes with left context through streaming_decode below; the incremental
-    # conv-buffer variant is SURVEY.md section 8f "next".
+    # ------------------------------------------------------------------ incremental (streaming) decode
+    # speech_tokenizer.py:882-930.  Every stateful layer reads one [B, H + rows, C] buffer: H history rows, then the rows of this call,
+    # which their producer writes in place (out= views), so the conv runs with pad_left = 0 over the whole buffer.  History rows hold
+    # pre-activation values (Snake stays in the conv prologue; it is elementwise, so this equals the reference's post-activation
+    # buffers).  Each buffer exists twice (ping-pong): the carry of the last H rows into the other copy's head is one launch for all
+    # layers, and stays race-free when the history is longer than a call's rows.  A decoder block's transposed conv writes its r-row
+    # overflow (bias included) past the rows of this call; the next call adds it, from the other copy, into its head rows -- the
+    # reference's overlap-add (DecoderBlockUpsample.step, :645-656), which counts the bias twice there.  The KV cache of the transformer
+    # is each layer's qkv buffer: the projection writes rows [offset, offset + L), RoPE and causal attention continue from offset.
+    kv_step = 256          # KV-cache capacity grows in steps of this many frames (the reference's KVCache step)
+
     def reset_streaming_state(self):
-        pass
+        """Start a new stream: the next ``streaming_step`` begins with empty conv history, KV cache and overlap buffers."""
+        self._st = None
+
+    def _stream_layers(self):
+        """(history rows, channels, rows per frame, overflow rows) of every buffered layer input, in the carry's order."""
+        W, cfg = self._w, self.config
+        layers = [(W["pre_conv"].K - 1, W["pre_conv"].cin, 1, 0)]
+        rpf = 1
+        for uw, f in zip(W["upsample"], cfg.upsampling_ratios):
+            if uw["up"].K != f:
+                raise NotImplementedError("streaming_step: an upsampling transposed conv with kernel != stride has no overlap buffer")
+            rpf *= f
+            layers.append((uw["dw"].K - 1, uw["dw"].cin, rpf, 0))
+        layers.append((W["init"].K - 1, W["init"].cin, rpf, 0))
+        for bw in W["blocks"]:
+            r = bw["r"]
+            if bw["up"].K != 2 * r:
+                raise NotImplementedError("streaming_step: decoder-block transposed convs must have kernel 2 * stride")
+            rpf *= r
+            for ui, u in enumerate(bw["units"]):
+                layers.append(((u["c1"].K - 1) * u["d"], u["c1"].cin, rpf, r if ui == 0 else 0))
+        layers.append((W["out_conv"].K - 1, W["out_conv"].cin, rpf, 0))
+        return layers
+
+    def _stream_buffers(self, B, cap):
+        layers = self._stream_layers()
+        return [[torch.zeros(B, H + cap * rpf + extra, C, device=self.device) for _ in range(2)] for (H, C, rpf, extra) in layers]
+
+    def _stream_grow(self, S, B, L):
+        """Make room for L new frames: conv buffers for chunks of L frames, KV capacity for offset + L (steps of ``kv_step``).  History,
+        overflow and cached K/V move to the new buffers in one launch each."""
+        layers = self._stream_layers()
+        if L > S["cap"]:
+            new = self._stream_buffers(B, L)
+            if S["off"] > 0:
+                p, q, moves = S["p"], 1 - S["p"], []
+                for (H, C, rpf, extra), old, nb in zip(layers, S["bufs"], new):
+                    moves.append((old[p][:, :H], nb[p][:, :H], False))
+                    if extra:
+                        t0 = H + S["prev"] * rpf
+                        moves.append((old[q][:, t0:t0 + extra], nb[q][:, t0:t0 + extra], False))
+                ops.stream_rows(moves)
+            S["bufs"], S["cap"] = new, L
+        need = S["off"] + L
+        if need > S["kv_cap"]:
+            cap = -(-need // self.kv_step) * self.kv_step
+            d3 = 3 * self.config.num_attention_heads * self.config.head_dim
+            new = [torch.empty(B, cap, d3, device=self.device) for _ in self._w["layers"]]
+            ops.stream_rows([(old[:, :S["off"]], nb[:, :S["off"]], False) for old, nb in zip(S["kv"], new)])
+            S["kv"], S["kv_cap"] = new, cap
+
+    @torch.no_grad()
+    def streaming_step(self, codes: torch.Tensor) -> torch.Tensor:
+        """codes int [B, num_quantizers, n_new] (only the new frames) -> audio [B, 1, 1920 n_new] clipped to [-1, 1], continuing the
+        stream begun by the last ``reset_streaming_state()`` (speech_tokenizer.py:889-930)."""
+        W, cfg, dev = self._w, self.config, self.device
+        if codes.shape[1] != cfg.num_quantizers:
+            raise ValueError(f"Expected {cfg.num_quantizers} layers of codes, got {codes.shape[1]}")
+        codes = codes.to(device=dev, dtype=torch.int64).contiguous()
+        B, nq, L = codes.shape
+        S = getattr(self, "_st", None)
+        if S is not None and S["B"] != B:
+            raise ValueError(f"streaming_step: batch size changed from {S['B']} to {B} within a stream (call reset_streaming_state first)")
+        if L == 0:
+            return torch.empty(B, 1, 0, device=dev)
+        if S is None:
+            S = self._st = {"B": B, "off": 0, "p": 0, "prev": 0, "cap": 0, "kv_cap": 0, "kv": [],
+                            "err": torch.zeros(1, dtype=torch.int32, device=dev)}
+        self._stream_grow(S, B, L)
+        layers = self._stream_layers()
+        p, off = S["p"], S["off"]
+        X = [b[p] for b in S["bufs"]]
+        prev = [b[1 - p] for b in S["bufs"]]
+        nsem = cfg.num_semantic_quantizers
+        H0 = layers[0][0]
+        pc_in = X[0][:, H0:H0 + L]
+        x = ops.conv1d(ops.rvq_decode(codes[:, :nsem], W["cb_first"], err=S["err"]), W["proj_first"], out=None if nq > nsem else pc_in)
+        if nq > nsem:
+            ops.conv1d(ops.rvq_decode(codes[:, nsem:], W["cb_rest"], err=S["err"]), W["proj_rest"], res=x, out=pc_in)
+        h = ops.conv1d(X[0][:, :H0 + L], W["pre_conv"], lout=L)
+        # ---- transformer with the KV cache (rows [0, off) of every layer's qkv buffer)
+        nh, hd, eps = cfg.num_attention_heads, cfg.head_dim, cfg.rms_norm_eps
+        d = nh * hd
+        x = ops.linear(h, W["in_proj"])
+        for lw, kv in zip(W["layers"], S["kv"]):
+            n = ops.layernorm(x, lw["n1"], None, eps=eps, rms=True)
+            new = kv[:, off:off + L]
+            ops.linear(n, lw["qkv"], out=new)
+            ops.rope_(new[:, :, :d], nh, offset=off, base=cfg.rope_theta, traditional=False)
+            ops.rope_(new[:, :, d:2 * d], nh, offset=off, base=cfg.rope_theta, traditional=False)
+            att = ops.attention(new[:, :, :d], kv[:, :off + L, d:2 * d], kv[:, :off + L, 2 * d:], n_heads=nh, scale=hd ** -0.5,
+                                causal=True, q_offset=off)
+            x = ops.linear(att, lw["o"], cscale=lw["ls1"], res=x)
+            n = ops.layernorm(x, lw["n2"], None, eps=eps, rms=True)
+            m = ops.swiglu(ops.linear(n, lw["gu"]))
+            x = ops.linear(m, lw["down"], cscale=lw["ls2"], res=x)
+        h = ops.linear(ops.layernorm(x, W["norm"], None, eps=eps, rms=True), W["out_proj"])
+        # ---- upsampling: transposed conv (k = s, no overlap) into the ConvNeXt buffer; pwconv2 writes the next buffered input
+        li = 1
+        for i, (uw, f) in enumerate(zip(W["upsample"], cfg.upsampling_ratios)):
+            Hh, rows = layers[li][0], h.shape[1] * f
+            cur = X[li][:, Hh:Hh + rows]
+            ops.conv1d(h, uw["up"], stride=f, pad_left=0, lout=rows, transpose=True, out=cur)
+            t = ops.conv1d(X[li][:, :Hh + rows], uw["dw"], lout=rows)
+            t = ops.layernorm(t, *uw["ln"], eps=1e-6)
+            t = ops.linear(t, uw["pw1"], post_act=ACT["gelu"])
+            nxt = X[li + 1][:, layers[li + 1][0]:layers[li + 1][0] + rows]
+            h = ops.linear(t, uw["pw2"], cscale=uw["gamma"], res=cur, out=nxt if i == len(W["upsample"]) - 1 else None)
+            li += 1
+        # ---- decoder: conv k7, 4 x (SnakeBeta, ConvT + overlap-add, 3 residual units), SnakeBeta, conv k7 -> 1, clip
+        Hh, rows = layers[li][0], h.shape[1]
+        w = ops.conv1d(X[li][:, :Hh + rows], W["init"], lout=rows)
+        li += 1
+        for bw in W["blocks"]:
+            r = bw["r"]
+            rows = w.shape[1] * r
+            H_, rpf = layers[li][0], layers[li][2]
+            ops.conv1d(w, bw["up"], stride=r, pad_left=0, lout=rows + r, pre=bw["snake"], transpose=True, out=X[li][:, H_:H_ + rows + r])
+            if off > 0:
+                t0 = H_ + S["prev"] * rpf
+                ops.stream_rows([(prev[li][:, t0:t0 + r], X[li][:, H_:H_ + r], True)])
+            for ui, u in enumerate(bw["units"]):
+                Hu = layers[li][0]
+                t = ops.conv1d(X[li][:, :Hu + rows], u["c1"], dilation=u["d"], lout=rows, pre=u["s1"])
+                Hn = layers[li + 1][0]
+                last_unit = ui == len(bw["units"]) - 1
+                out = X[li + 1][:, Hn:Hn + rows] if (not last_unit or bw is W["blocks"][-1]) else None
+                w = ops.conv1d(t, u["c2"], pre=u["s2"], res=X[li][:, Hu:Hu + rows], out=out)
+                li += 1
+        Hh, rows = layers[li][0], w.shape[1]
+        wav = ops.conv1d(X[li][:, :Hh + rows], W["out_conv"], lout=rows, pre=W["out_snake"], post_act=ACT["clip1"])
+        # ---- carry: the last H rows of every buffered input become the other copy's history head (one launch)
+        carry = []
+        for (H, C, rpf, extra), buf, nb in zip(layers, X, prev):
+            end = H + L * rpf
+            carry.append((buf[:, end - H:end], nb[:, :H], False))
+        ops.stream_rows(carry)
+        S["p"], S["off"], S["prev"] = 1 - p, off + L, L
+        return wav.reshape(B, 1, -1)
 
 
 class Qwen3TTSSpeechTokenizer:
