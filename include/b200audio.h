@@ -386,6 +386,46 @@ typedef struct {
  * any range another entry reads or writes (B2A_E_INVALID otherwise).  Empty entries are skipped. */
 int32_t b2a_stream_rows(const b2a_rowop_t* ops, int32_t n, void* stream);
 
+/* ---- Qwen3-TTS speaker encoder (ECAPA-TDNN, tts/models/qwen3_tts/speaker_encoder.py) and its log-mel front end -------------- */
+/* qwen3_tts.py:64-121 (mel_spectrogram): reflect pad of (1024-256)/2 samples (no repeated edge), STFT (n_fft 1024, hop 256,
+ * center=False, periodic Hann `window`), sqrt(|X|^2 + 1e-9) @ filters^T (Slaney mel, [n_mels, 513]), log(max(., 1e-5)).
+ * x [B, n] (row stride x_bs), n > 384; out [B, frames, n_mels] contiguous with frames = 1 + (n + 768 - 1024) / 256. */
+int32_t b2a_spk_logmel(const float* x, int64_t x_bs, int32_t B, int64_t n, const float* window, const float* filters, int32_t n_mels,
+                       int64_t frames, float* out, void* stream);
+/* speaker_encoder.py:11-26 (reflect_pad_1d) as the operand of the following conv, which then runs unpadded: x [B, T, C] ->
+ * rows reflect(r - pad) for r in [0, T + 2 pad), either fp32 out_f32 [B, T+2pad, C] contiguous, or the tensor-core conv's bf16
+ * planes hi / lo (lo may be NULL) [B, T+2pad, cpad] with zeroed pad channels.  Exactly one of out_f32 / hi; pad < T. */
+int32_t b2a_spk_reflect_pad(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T, int32_t C, int32_t pad, float* out_f32,
+                            void* hi, void* lo, int32_t cpad, void* stream);
+/* speaker_encoder.py:60-101 (Res2NetBlock, with the TimeDelayNetBlocks of :29-57): y [B, T, scale*C] -> z [B, T, scale*C]; chunk 0
+ * copied, chunk i = relu(conv(reflect_pad(chunk_i + chunk_{i-1}' ))) for i >= 1 (chunk 1 without the add) -- the whole dependent chain
+ * in one launch, one CTA per (item, `tile` rows), halo recomputed.  w [scale-1][K][C_in][C_out] fp32, bias [scale-1][C];
+ * (K-1)*dilation even, pad = (K-1)*dilation/2 < T.  Shared memory per CTA: b2a_spk_res2net_smem_bytes (B2A_E_UNSUPPORTED > 227 KB). */
+int64_t b2a_spk_res2net_smem_bytes(int32_t C, int32_t scale, int32_t K, int32_t pad, int32_t tile);
+int32_t b2a_spk_res2net(const float* y, int64_t y_bs, int64_t y_ld, float* z, int64_t z_bs, int64_t z_ld, const float* w, const float* bias,
+                        int32_t B, int32_t T, int32_t C, int32_t scale, int32_t K, int32_t dilation, int32_t tile, void* stream);
+/* Per-channel mean over T (speaker_encoder.py:127, :191) and, with_std, sqrt(var + eps) (:192, biased var) of x [B, T, C]:
+ * out[b*o_bs + c] = mean, out[b*o_bs + C + c] = std.  Fixed summation order (bit-reproducible). */
+int32_t b2a_spk_channel_stats(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T, int32_t C, int32_t with_std, float eps,
+                              float* out, int64_t o_bs, void* stream);
+/* speaker_encoder.py:124-133 after the mean: gate[b] = sigmoid(w2 relu(w1 mean[b] + b1) + b2); w1 [S, C], w2 [C, S]; gate [B, C]. */
+int32_t b2a_spk_se_gate(const float* mean, int64_t m_bs, int32_t B, int32_t C, int32_t S, const float* w1, const float* b1, const float* w2,
+                        const float* b2, float* gate, void* stream);
+/* speaker_encoder.py:133,168: out = y * gate[b, c] + res (out may be a channel slice of the MFA concatenation, :293-295). */
+int32_t b2a_spk_se_apply(const float* y, int64_t y_bs, int64_t y_ld, const float* gate, const float* res, int64_t r_bs, int64_t r_ld,
+                         float* out, int64_t o_bs, int64_t o_ld, int32_t B, int32_t T, int32_t C, void* stream);
+/* One row per item: y[b*y_bs + j] = act(bias[j] + w[j*w_ld : +K] . x[b*x_bs : +K]) (act: B2A_ACT_*; LRELU means ReLU).  The statistics
+ * half of the pooling TDNN (:177,202) and the final 1x1 projection (:269-303). */
+int32_t b2a_spk_gemv(const float* x, int64_t x_bs, int32_t B, int32_t K, const float* w, int64_t w_ld, int32_t N, const float* bias,
+                     int32_t act, float* y, int64_t y_bs, void* stream);
+/* speaker_encoder.py:202-203 with the TDNN split as W_x.x + (W_m.mean + W_s.std + b): h = tanh(relu(h + cb[b])) in place, h [B, T, A],
+ * cb [B, A] contiguous. */
+int32_t b2a_spk_asp_act(float* h, int64_t h_bs, int64_t h_ld, const float* cb, int32_t B, int32_t T, int32_t A, void* stream);
+/* speaker_encoder.py:208-216: softmax over TIME of logits [B, T, C] per channel (max-subtracted), weighted mean of x [B, T, C] and
+ * sqrt(max(weighted var, eps)) -> pooled[b*p_bs + c] = mean, pooled[b*p_bs + C + c] = std.  Fixed summation order. */
+int32_t b2a_spk_asp_pool(const float* logits, int64_t l_bs, int64_t l_ld, const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T,
+                         int32_t C, float eps, float* pooled, int64_t p_bs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

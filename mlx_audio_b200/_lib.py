@@ -123,6 +123,16 @@ PROTOTYPES = {
     "b2a_snac_from_codes": (i32, [C.POINTER(C.c_void_p), C.POINTER(i32), i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                   C.POINTER(C.c_void_p), i32, i64, i32, i32, i32, c_f, c_f, C.c_void_p]),
     "b2a_stream_rows": (i32, [C.POINTER(RowOp), i32, C.c_void_p]),
+    "b2a_spk_logmel": (i32, [c_f, i64, i32, i64, c_f, c_f, i32, i64, c_f, C.c_void_p]),
+    "b2a_spk_reflect_pad": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, c_f, i32, C.c_void_p]),
+    "b2a_spk_res2net_smem_bytes": (i64, [i32, i32, i32, i32, i32]),
+    "b2a_spk_res2net": (i32, [c_f, i64, i64, c_f, i64, i64, c_f, c_f, i32, i32, i32, i32, i32, i32, i32, C.c_void_p]),
+    "b2a_spk_channel_stats": (i32, [c_f, i64, i64, i32, i32, i32, i32, f32, c_f, i64, C.c_void_p]),
+    "b2a_spk_se_gate": (i32, [c_f, i64, i32, i32, i32, c_f, c_f, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_spk_se_apply": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, C.c_void_p]),
+    "b2a_spk_gemv": (i32, [c_f, i64, i32, i32, c_f, i64, i32, c_f, i32, c_f, i64, C.c_void_p]),
+    "b2a_spk_asp_act": (i32, [c_f, i64, i64, c_f, i32, i32, i32, C.c_void_p]),
+    "b2a_spk_asp_pool": (i32, [c_f, i64, i64, c_f, i64, i64, i32, i32, i32, f32, c_f, i64, C.c_void_p]),
 }
 
 E_INVALID, E_CUDA, E_UNSUPPORTED = -1, -2, -3

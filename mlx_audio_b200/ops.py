@@ -1083,3 +1083,122 @@ def snac_from_codes(codes, strides, embs, ws, biases, dim: int, check=True) -> t
     if check and int(err.item()) != 0:
         raise ValueError(f"snac_from_codes: code index out of range [0, {bins})")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------- speaker encoder
+def spk_logmel(x: torch.Tensor, window: torch.Tensor, filters: torch.Tensor) -> torch.Tensor:
+    """Qwen3-TTS speaker log-mel (qwen3_tts.py:64-121): x [B, n] float32 -> [B, frames, n_mels]; ``window`` [1024], ``filters`` [n_mels, 513]."""
+    B, n = x.shape
+    assert x.dtype == torch.float32 and x.stride(1) == 1 and window.numel() == 1024 and filters.is_contiguous() and filters.shape[1] == 513
+    if n <= 384:
+        raise ValueError(f"speaker log-mel: the reflect padding of 384 samples needs more than 384 samples, got {n}")
+    frames = 1 + (n + 768 - 1024) // 256
+    out = torch.empty(B, frames, filters.shape[0], device=x.device, dtype=torch.float32)
+    _call("logmel", _lib.lib().b2a_spk_logmel, 1, x.data_ptr(), x.stride(0), B, n, window.data_ptr(), filters.data_ptr(), filters.shape[0],
+          frames, out.data_ptr(), _stream())
+    return out
+
+
+def spk_reflect_pad(x: torch.Tensor, pad: int, cpad: int = 0, planes: int = 2):
+    """Reflect "same" padding (speaker_encoder.py:11-26) written as the next conv's operand: ``cpad`` 0 -> fp32 [B, T+2pad, C];
+    otherwise the bf16 ``Planes`` [B, T+2pad, cpad] of the tensor-core conv (``planes`` 1: hi only)."""
+    _chk3(x, "spk_reflect_pad x")
+    B, T, Cc = x.shape
+    if pad >= T:
+        raise ValueError(f"reflect padding of {pad} rows needs more than {pad} frames, got {T}")
+    if cpad:
+        pl = Planes(torch.empty(B, T + 2 * pad, cpad, device=x.device, dtype=torch.bfloat16),
+                    torch.empty(B, T + 2 * pad, cpad, device=x.device, dtype=torch.bfloat16) if planes == 2 else None, Cc)
+        _call("prep", _lib.lib().b2a_spk_reflect_pad, 1, x.data_ptr(), x.stride(0), x.stride(1), B, T, Cc, pad, None, pl.hi.data_ptr(),
+              _p(pl.lo), cpad, _stream())
+        return pl
+    out = torch.empty(B, T + 2 * pad, Cc, device=x.device, dtype=torch.float32)
+    _call("prep", _lib.lib().b2a_spk_reflect_pad, 1, x.data_ptr(), x.stride(0), x.stride(1), B, T, Cc, pad, out.data_ptr(), None, None, 0,
+          _stream())
+    return out
+
+
+SPK_RES2NET_TILE = 32      # output rows per CTA of the Res2Net chain (halo (scale-1)*pad rows per side is recomputed)
+
+
+def spk_res2net(y: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, scale: int, dilation: int, out=None, tile: int = 0) -> torch.Tensor:
+    """Res2NetBlock (speaker_encoder.py:60-101) in one launch: y [B, T, scale*C] -> [B, T, scale*C]; ``w`` [scale-1, K, C, C]
+    (stage, tap, in, out), ``bias`` [scale-1, C]."""
+    _chk3(y, "spk_res2net y")
+    B, T, CC = y.shape
+    S1, K, Cc, _ = w.shape
+    assert S1 == scale - 1 and CC == scale * Cc and w.is_contiguous() and bias.is_contiguous() and w.dtype == torch.float32
+    pad = (K - 1) * dilation // 2
+    if pad >= T:
+        raise ValueError(f"Res2Net: reflect padding of {pad} rows needs more than {pad} frames, got {T}")
+    if out is None:
+        out = torch.empty(B, T, CC, device=y.device, dtype=torch.float32)
+    _chk3(out, "spk_res2net out")
+    _call("other", _lib.lib().b2a_spk_res2net, 1, y.data_ptr(), y.stride(0), y.stride(1), out.data_ptr(), out.stride(0), out.stride(1),
+          w.data_ptr(), bias.data_ptr(), B, T, Cc, scale, K, dilation, tile or SPK_RES2NET_TILE, _stream())
+    return out
+
+
+def spk_channel_stats(x: torch.Tensor, with_std: bool, eps: float = 1e-12, out=None) -> torch.Tensor:
+    """Per-channel mean over T of x [B, T, C] -> [B, C], or [B, 2C] = (mean | sqrt(var + eps)) with ``with_std``; fixed order."""
+    _chk3(x, "spk_channel_stats x")
+    B, T, Cc = x.shape
+    if out is None:
+        out = torch.empty(B, (2 if with_std else 1) * Cc, device=x.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_spk_channel_stats, 1, x.data_ptr(), x.stride(0), x.stride(1), B, T, Cc, int(with_std), eps,
+          out.data_ptr(), out.stride(0), _stream())
+    return out
+
+
+def spk_se_gate(mean: torch.Tensor, w1, b1, w2, b2) -> torch.Tensor:
+    """sigmoid(w2 relu(w1 mean + b1) + b2) per item: mean [B, C], w1 [S, C], w2 [C, S] -> gate [B, C]."""
+    B, Cc = mean.shape
+    S = w1.shape[0]
+    assert mean.stride(1) == 1 and w1.is_contiguous() and w2.is_contiguous() and tuple(w2.shape) == (Cc, S)
+    gate = torch.empty(B, Cc, device=mean.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_spk_se_gate, 1, mean.data_ptr(), mean.stride(0), B, Cc, S, w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
+          b2.data_ptr(), gate.data_ptr(), _stream())
+    return gate
+
+
+def spk_se_apply(y: torch.Tensor, gate: torch.Tensor, res: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out = y * gate[b, c] + res (all [B, T, C] row-strided views)."""
+    for t, n in ((y, "y"), (res, "res"), (out, "out")):
+        _chk3(t, "spk_se_apply " + n)
+    B, T, Cc = y.shape
+    assert res.shape == y.shape and out.shape == y.shape and gate.is_contiguous() and tuple(gate.shape) == (B, Cc)
+    _call("other", _lib.lib().b2a_spk_se_apply, 1, y.data_ptr(), y.stride(0), y.stride(1), gate.data_ptr(), res.data_ptr(), res.stride(0),
+          res.stride(1), out.data_ptr(), out.stride(0), out.stride(1), B, T, Cc, _stream())
+    return out
+
+
+def spk_gemv(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, act: int = 0) -> torch.Tensor:
+    """y[b] = act(w x[b] + bias): x [B, K] (unit column stride), w [N, K] fp32 (row-strided) -> [B, N]."""
+    B, K = x.shape
+    N = w.shape[0]
+    assert x.stride(1) == 1 and w.stride(1) == 1 and w.shape[1] == K and x.dtype == w.dtype == torch.float32
+    y = torch.empty(B, N, device=x.device, dtype=torch.float32)
+    _call("gemv", _lib.lib().b2a_spk_gemv, 1, x.data_ptr(), x.stride(0), B, K, w.data_ptr(), w.stride(0), N, _p(bias), act, y.data_ptr(),
+          y.stride(0), _stream())
+    return y
+
+
+def spk_asp_act(h: torch.Tensor, cb: torch.Tensor) -> torch.Tensor:
+    """In place: h = tanh(relu(h + cb[b])), h [B, T, A], cb [B, A]."""
+    _chk3(h, "spk_asp_act h")
+    B, T, A = h.shape
+    assert cb.is_contiguous() and tuple(cb.shape) == (B, A)
+    _call("other", _lib.lib().b2a_spk_asp_act, 1, h.data_ptr(), h.stride(0), h.stride(1), cb.data_ptr(), B, T, A, _stream())
+    return h
+
+
+def spk_asp_pool(logits: torch.Tensor, x: torch.Tensor, eps: float = 1e-12) -> torch.Tensor:
+    """Softmax over time per channel + weighted mean / std (speaker_encoder.py:208-216): logits, x [B, T, C] -> [B, 2C] (mean | std)."""
+    _chk3(logits, "spk_asp_pool logits")
+    _chk3(x, "spk_asp_pool x")
+    B, T, Cc = x.shape
+    assert logits.shape == x.shape
+    out = torch.empty(B, 2 * Cc, device=x.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_spk_asp_pool, 1, logits.data_ptr(), logits.stride(0), logits.stride(1), x.data_ptr(), x.stride(0),
+          x.stride(1), B, T, Cc, eps, out.data_ptr(), out.stride(0), _stream())
+    return out

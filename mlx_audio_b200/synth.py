@@ -533,3 +533,32 @@ def qwen3_tokenizer_weights(cfg, seed=12):
 def qwen3_codes(cfg, t, batch=1, seed=13):
     """codes [B, 16, T] (first code > 0 so that the valid-length rule of speech_tokenizer.py:1113-1116 keeps every frame)."""
     return torch.randint(1, cfg["codebook_size"], (batch, cfg["num_quantizers"], t), generator=torch.Generator().manual_seed(seed))
+
+
+def qwen3_speaker_encoder_weights(cfg, seed=14):
+    """Parameter tree of tts/models/qwen3_tts/speaker_encoder.py:Qwen3TTSSpeakerEncoder with the checkpoint's ``speaker_encoder.``
+    prefix, MLX conv layout [out, K, in]; ``cfg`` is a dict of oracle/qwen3.py:SPEAKER_ENCODER's keys.  bf16-exact values, weights
+    scaled by 1/sqrt(fan-in) so that every block's activations stay O(1), biases N(0, 0.05)."""
+    g = _Gen(seed)
+    ch, ks, sc = cfg["enc_channels"], cfg["enc_kernel_sizes"], cfg["enc_res2net_scale"]
+    A, S, E = cfg["enc_attention_channels"], cfg["enc_se_channels"], cfg["enc_dim"]
+
+    def conv(name, cout, k, cin):
+        g.normal(name + ".weight", cout, k, cin, std=1.0 / math.sqrt(k * cin))
+        g.normal(name + ".bias", cout, std=0.05)
+
+    p = "speaker_encoder."
+    conv(p + "blocks.0.conv", ch[0], ks[0], cfg["mel_dim"])
+    for i in range(1, len(ch) - 1):
+        b = f"{p}blocks.{i}"
+        conv(b + ".tdnn1.conv", ch[i], 1, ch[i - 1])
+        for j in range(sc - 1):
+            conv(f"{b}.res2net_block.blocks.{j}.conv", ch[i] // sc, ks[i], ch[i] // sc)
+        conv(b + ".tdnn2.conv", ch[i], 1, ch[i])
+        conv(b + ".se_block.conv1", S, 1, ch[i])
+        conv(b + ".se_block.conv2", ch[i], 1, S)
+    conv(p + "mfa.conv", ch[-1], ks[-1], sum(ch[1:-1]))
+    conv(p + "asp.tdnn.conv", A, 1, 3 * ch[-1])
+    conv(p + "asp.conv", ch[-1], 1, A)
+    conv(p + "fc", E, 1, 2 * ch[-1])
+    return g.P

@@ -1,7 +1,7 @@
 """Qwen3-TTS generation loop on H100 (reference: tts/models/qwen3_tts/qwen3_tts.py).
 
 Covers the base path of ``Model.generate`` (qwen3_tts.py:1122-1575): input assembly from token ids
-(``_prepare_generation_inputs`` :326-484 minus the tokenizer / speaker encoder, which are host / "next" rows), the per-frame
+(``_prepare_generation_inputs`` :326-484 after the host tokenizer, with x-vector cloning through ``speaker_encoder.py``), the per-frame
 loop (:1323-1404) with ``_sample_token`` (:805-860), and ``_decode_chunk`` (:1017-1048) through the speech tokenizer.
 
 One frame = talker step + first-codebook sample + 15 code-predictor sub-steps (each with its sampler) + next-input
@@ -19,6 +19,7 @@ import torch
 from .... import ops
 from ..base import GenerationResult
 from .config import ModelConfig
+from .speaker_encoder import Qwen3TTSSpeakerEncoder
 from .speech_tokenizer import Qwen3TTSSpeechTokenizer
 from .talker import Qwen3TTSTalkerForConditionalGeneration
 
@@ -32,23 +33,30 @@ def format_duration(seconds: float) -> str:
     return f"{hours:02d}:{minutes:02d}:{secs:02d}.{ms:03d}"
 
 
+_MEL_CACHE = {}
+
+
 def mel_spectrogram(audio, n_fft: int = 1024, num_mels: int = 128, sample_rate: int = 24000, hop_size: int = 256,
                     win_size: int = 1024, fmin: float = 0.0, fmax: float = 12000.0, device="cuda") -> torch.Tensor:
     """qwen3_tts.py:64-120 (speaker-encoder front end): manual reflect pad of (n_fft-hop)/2, STFT (center=False, Hann),
-    sqrt(|X|^2 + 1e-9) @ slaney-mel^T, log(clip(., 1e-5)).  [n] or [B, n] -> [B, frames, num_mels]; the batch is one STFT launch."""
+    sqrt(|X|^2 + 1e-9) @ slaney-mel^T, log(clip(., 1e-5)).  [n] or [B, n] -> [B, frames, num_mels]: one launch for the batch
+    (``ops.spk_logmel``), which implements the speaker encoder's configuration (1024 / 256 / 1024) only."""
     from .... import dsp
-    a = torch.as_tensor(audio, dtype=torch.float32, device=device)
+    if (n_fft, hop_size, win_size) != (1024, 256, 1024):
+        raise NotImplementedError("mel_spectrogram: the speaker log-mel kernel covers n_fft = win_size = 1024, hop_size = 256")
+    on_dev = isinstance(audio, torch.Tensor) and audio.is_cuda
+    a = (audio.float() if on_dev else torch.as_tensor(audio, dtype=torch.float32)).to(device)          # host samples: one copy in
     if a.dim() == 1:
         a = a[None]
-    pad = (n_fft - hop_size) // 2
-    a = torch.cat([a[:, 1:pad + 1].flip(1), a, a[:, -(pad + 1):-1].flip(1)], dim=1)
-    spec = dsp.stft(a, n_fft=n_fft, hop_length=hop_size, win_length=win_size, window="hann", center=False, pad_mode="reflect", device=device)
-    mag = torch.sqrt(spec.real ** 2 + spec.imag ** 2 + 1e-9)
-    basis = dsp.mel_filters(sample_rate=sample_rate, n_fft=n_fft, n_mels=num_mels, f_min=fmin, f_max=fmax, norm="slaney", mel_scale="slaney")
-    basis = torch.as_tensor(basis, dtype=torch.float32, device=a.device)
-    cw = ops.pack_linear(basis, None, a.device)
-    mel = ops.linear(mag.contiguous(), cw)
-    return torch.log(torch.clamp(mel, min=1e-5))
+    a = a.contiguous()
+    key = (a.device, num_mels, sample_rate, float(fmin), float(fmax))
+    if key not in _MEL_CACHE:
+        basis = dsp.mel_filters(sample_rate=sample_rate, n_fft=n_fft, n_mels=num_mels, f_min=fmin, f_max=fmax, norm="slaney", mel_scale="slaney")
+        window = dsp._resolve_window("hann", win_size)
+        _MEL_CACHE[key] = (torch.as_tensor(window, dtype=torch.float32).to(a.device).contiguous(),
+                           torch.as_tensor(basis, dtype=torch.float32).to(a.device).contiguous())
+    window, basis = _MEL_CACHE[key]
+    return ops.spk_logmel(a, window, basis)
 
 
 class Model:
@@ -56,7 +64,11 @@ class Model:
         self.config = config
         self.device = torch.device(device)
         self.talker = Qwen3TTSTalkerForConditionalGeneration(config.talker_config, device)
-        self.speaker_encoder = None          # ECAPA-TDNN voice cloning: SURVEY.md section 8f "next"
+        # ECAPA-TDNN speaker encoder for x-vector voice cloning: base models only, as in the reference (qwen3_tts.py:178-182)
+        self.speaker_encoder = Qwen3TTSSpeakerEncoder(config.speaker_encoder_config, device) \
+            if getattr(config, "tts_model_type", "base") == "base" else None
+        self.talker_dtype = torch.float32     # the talker checkpoint's dtype (weights are held in fp32; the x-vector is rounded to it)
+        self.speech_tokenizer_has_encoder = False   # speech_tokenizer/config.json has an encoder_config (the ICL route's condition)
         self.speech_tokenizer: Optional[Qwen3TTSSpeechTokenizer] = None
         self.tokenizer = None
         self.generate_config = None
@@ -82,7 +94,14 @@ class Model:
     def load_weights(self, weights, strict: bool = True):
         """``weights`` (dict or list of pairs) with the checkpoint's ``talker.`` prefix (stripped here, talker.py:825-839)."""
         weights = dict(weights)
-        self.talker.load_weights(self.talker.sanitize(weights))
+        talker_w = self.talker.sanitize(weights)
+        floats = [v.dtype for v in talker_w.values() if isinstance(v, torch.Tensor) and v.is_floating_point()]
+        if floats:
+            self.talker_dtype = floats[0]
+        self.talker.load_weights(talker_w)
+        spk = {k: v for k, v in weights.items() if k.startswith("speaker_encoder.")}
+        if self.speaker_encoder is not None and spk:
+            self.speaker_encoder.load_weights(self.speaker_encoder.sanitize(spk))
         t = self.talker
         self._tabs_all = ops.EmbedTables([t.codec_embedding] + t.code_predictor.codec_embedding)
         self._tab0 = ops.EmbedTables([t.codec_embedding])
@@ -127,6 +146,7 @@ class Model:
         if st_path.exists():
             from safetensors.torch import load_file
             d = json.load(open(st_path / "config.json"))
+            model.speech_tokenizer_has_encoder = "encoder_config" in d       # speech_tokenizer.py:1076-1097, read at qwen3_tts.py:2838-2854
             dec = Qwen3TTSTokenizerDecoderConfig(**filter_dict_for_dataclass(Qwen3TTSTokenizerDecoderConfig, d["decoder_config"])) \
                 if "decoder_config" in d else None
             tc = Qwen3TTSTokenizerConfig(decoder_config=dec)
@@ -158,6 +178,9 @@ class Model:
         tts_bos, tts_eos, tts_pad = tts[:, 0:1], tts[:, 1:2], tts[:, 2:3]
         if speaker_embed is None and speaker_id is not None:
             speaker_embed = ops.gather_rows(t.codec_embedding, torch.tensor([int(speaker_id)], device=dev))[None]
+        elif speaker_embed is not None and self.talker_dtype != torch.float32:
+            # the speaker encoder runs in fp32; the reference casts its output to the talker's dtype before the prefix (qwen3_tts.py:429-432)
+            speaker_embed = torch.as_tensor(speaker_embed, device=dev).to(self.talker_dtype)
         if language_id is None:
             prefill = [cfg.codec_nothink_id, cfg.codec_think_bos_id, cfg.codec_think_eos_id]
         else:
@@ -177,8 +200,21 @@ class Model:
         trailing = torch.cat([text_embed[:, 4:-5], tts_eos], dim=1).contiguous()
         return input_embeds, trailing, tts_pad.contiguous()
 
-    def _prepare_generation_inputs(self, text: str, language: str = "auto", speaker: Optional[str] = None, instruct: Optional[str] = None):
-        """qwen3_tts.py:326-484: tokenise with the chat template, resolve speaker / language / dialect ids from the config."""
+    def extract_speaker_embedding(self, audio, sr: int = 24000) -> torch.Tensor:
+        """qwen3_tts.py:285-324: 24 kHz samples [n] or [B, n] -> x-vector [B, enc_dim] (float32): log-mel front end + ECAPA-TDNN."""
+        if sr != 24000:
+            raise ValueError("Only 24kHz audio is supported for speaker embedding extraction")
+        if self.speaker_encoder is None:
+            raise ValueError("Speaker encoder not available for this model type")
+        mels = mel_spectrogram(audio, n_fft=1024, num_mels=128, sample_rate=24000, hop_size=256, win_size=1024, fmin=0, fmax=12000,
+                               device=self.device)
+        return self.speaker_encoder(mels)
+
+    def _prepare_generation_inputs(self, text: str, language: str = "auto", speaker: Optional[str] = None, instruct: Optional[str] = None,
+                                   ref_audio=None):
+        """qwen3_tts.py:326-484: tokenise with the chat template, resolve speaker / language / dialect ids from the config; with
+        ``ref_audio`` (base models) the x-vector of the reference audio takes the speaker row (it wins over ``speaker``, whose dialect
+        override still applies)."""
         if self.tokenizer is None:
             raise ValueError("Tokenizer not loaded. Call post_load_hook first.")
         cfg = self.config.talker_config
@@ -196,7 +232,10 @@ class Model:
             if dialect in (cfg.codec_language_id or {}):
                 language_id = cfg.codec_language_id[dialect]
         instruct_ids = self.tokenizer.encode(f"<|im_start|>user\n{instruct}<|im_end|>\n") if instruct else None
-        return self.prepare_generation_inputs_from_ids(ids, language_id, speaker_id, instruct_ids=instruct_ids)
+        speaker_embed = None
+        if ref_audio is not None and self.speaker_encoder is not None:
+            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        return self.prepare_generation_inputs_from_ids(ids, language_id, speaker_id, speaker_embed=speaker_embed, instruct_ids=instruct_ids)
 
     def _suppress_codec_tokens(self, eos_token_id: int):
         """qwen3_tts.py:927-933."""
@@ -494,13 +533,18 @@ class Model:
 
     def generate_from_ids(self, input_ids, *, language_id=None, speaker_id=None, temperature: float = 0.9, max_tokens: int = 4096,
                           top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, seed: int = 0, u=None,
-                          stream: bool = False, streaming_interval: float = 2.0, **kwargs):
+                          stream: bool = False, streaming_interval: float = 2.0, ref_audio=None, speaker_embed=None, **kwargs):
         """``Model.generate`` (qwen3_tts.py:1122-1575) for one already-tokenised segment; yields one GenerationResult, or with
-        ``stream=True`` one per ``streaming_interval`` seconds of generated frames (the last with ``is_final_chunk``)."""
+        ``stream=True`` one per ``streaming_interval`` seconds of generated frames (the last with ``is_final_chunk``).  ``ref_audio``
+        (24 kHz samples, base models) = x-vector cloning: its speaker embedding takes the speaker row, as ``speaker_embed`` [1, H] does."""
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
-        x, trailing, pad = self.prepare_generation_inputs_from_ids(input_ids, language_id, speaker_id)
+        if ref_audio is not None:
+            if self.speaker_encoder is None:
+                raise ValueError("Speaker encoder not available for this model type")
+            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        x, trailing, pad = self.prepare_generation_inputs_from_ids(input_ids, language_id, speaker_id, speaker_embed=speaker_embed)
         if stream:
             yield from self._stream_segment(x, trailing, pad, 0, streaming_interval, dict(
                 max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u))
@@ -520,14 +564,14 @@ class Model:
                                audio_samples={"samples": samples, "samples-per-sec": round(samples / dt, 2) if dt > 0 else 0},
                                processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
 
-    def _generate_segments(self, text, split_pattern, speaker, language, instruct, stream=False, streaming_interval=2.0, **gen):
+    def _generate_segments(self, text, split_pattern, speaker, language, instruct, stream=False, streaming_interval=2.0, ref_audio=None, **gen):
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         # base path: segments are split AND stripped (qwen3_tts.py:1268-1271); the instruct paths pass split_pattern=None and the text as is
         segments = [t.strip() for t in text.split(split_pattern) if t.strip()] if split_pattern else [text]
         for idx, seg in enumerate(segments):
             t0 = time.perf_counter()
-            x, trailing, pad = self._prepare_generation_inputs(seg, language=language, speaker=speaker, instruct=instruct)
+            x, trailing, pad = self._prepare_generation_inputs(seg, language=language, speaker=speaker, instruct=instruct, ref_audio=ref_audio)
             seg_gen = dict(gen)
             if seg_gen.get("seed") is not None:                       # a fixed seed still gives every segment its own draws
                 seg_gen["seed"] = int(seg_gen["seed"]) + idx
@@ -570,12 +614,13 @@ class Model:
             return
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
-        if ref_audio is not None:
-            # with ref_text: in-context cloning (_generate_icl); alone: x-vector cloning through the speaker encoder (qwen3_tts.py:382-383).
-            # Neither encoder has a CUDA path yet -- refuse instead of silently synthesising the default voice.
-            raise NotImplementedError("voice cloning from ref_audio needs the speech-tokenizer encoder + speaker encoder "
-                                      "(SURVEY.md section 8f 'next'); call without ref_audio for the default voice")
+        if ref_audio is not None and ref_text is not None and self.speech_tokenizer_has_encoder:
+            # in-context cloning (_generate_icl, qwen3_tts.py:1233-1256): needs the speech-tokenizer encoder, which has no CUDA path yet --
+            # refuse instead of silently synthesising another voice
+            raise NotImplementedError("in-context (ICL) voice cloning from ref_audio + ref_text is not implemented; pass ref_audio "
+                                      "without ref_text for x-vector cloning")
         if voice is not None and voice.lower() not in [s.lower() for s in self.supported_speakers]:
             raise ValueError(f"Voice '{voice}' is not supported by this Base model. Base models have no built-in preset voices — "
                              "clone a voice by passing ref_audio and ref_text instead.")
-        yield from self._generate_segments(text, split_pattern, voice, lang_code, None, stream, streaming_interval, **gen)
+        # ref_audio alone (or with ref_text when the speech tokenizer has no encoder): x-vector cloning on every segment (:381-383)
+        yield from self._generate_segments(text, split_pattern, voice, lang_code, None, stream, streaming_interval, ref_audio=ref_audio, **gen)
