@@ -326,6 +326,15 @@ int32_t b2a_attn_decode(const float* q, int64_t q_bs, int64_t q_ss, const float*
                         int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
                         int32_t D, float scale, const int32_t* base_dev, int32_t base_host, const int32_t* kv_start,
                         int32_t max_k, void* stream);
+/* The same contract as b2a_attn_decode for long prefills (talker.py:288-312 over a prompt of >= 64 rows: the in-context voice-cloning
+ * prompt) on the tensor cores: head_dim 128, Hq = 2 Hkv.  One CTA per (64 query rows, kv head, batch row); both query heads of the GQA
+ * pair share each K / V tile, which is read once from the fp32 cache and split into fp16 hi / lo planes (3-product scores and P V,
+ * fp32 accumulate).  Keys are taken in a fixed order: bit-reproducible.  Query row s sees cache rows [kv_start[b], min(base + s,
+ * max_k - 1)].  Rows 16-byte aligned (q, caches); out rows 8-byte aligned. */
+int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, const float* k_cache, const float* v_cache, int64_t c_bs,
+                         int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
+                         int32_t D, float scale, const int32_t* base_dev, int32_t base_host, const int32_t* kv_start,
+                         int32_t max_k, void* stream);
 /* Single-token decode (S = 1, GQA group of 2): b2a_qknorm_rope_cache + b2a_attn_decode in one launch, one CTA per (kv head, batch)
  * -- each cache row is read once for both query heads of the group.  qkv [B, (Hq+2Hkv) D]; out [B, Hq*D]; pos3 [3,B] or NULL. */
 int32_t b2a_attn_decode_fused(const float* qkv, int64_t qkv_bs, int32_t B, int32_t Hq, int32_t Hkv, int32_t D, const float* q_norm_w,

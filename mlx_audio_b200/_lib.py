@@ -113,6 +113,7 @@ PROTOTYPES = {
     "b2a_qknorm_rope_cache": (i32, [c_f, i64, i64, i32, i32, i32, i32, i32, c_f, c_f, f32, c_f, c_f, i32, i32, i32, f32, c_f, i64, i64,
                                     c_f, c_f, i64, i64, i32, c_f, C.c_void_p]),
     "b2a_attn_decode": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, C.c_void_p]),
+    "b2a_attn_prefill": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, C.c_void_p]),
     "b2a_attn_decode_fused": (i32, [c_f, i64, i32, i32, i32, i32, c_f, c_f, f32, c_f, c_f, i32, i32, i32, f32, c_f, c_f, i64, i64, i32, f32,
                                     c_f, c_f, i64, C.c_void_p]),
     "b2a_swiglu": (i32, [c_f, i64, i64, i32, i32, c_f, i64, C.c_void_p]),

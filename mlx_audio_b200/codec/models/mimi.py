@@ -166,19 +166,6 @@ class Mimi:
         W["proj_first"] = ops.pack_conv(P["quantizer.rvq_first.output_proj.weight"].float(), None, 1, dev)
         W["proj_rest"] = ops.pack_conv(P["quantizer.rvq_rest.output_proj.weight"].float(), None, 1, dev) if cfg.nq > 1 else None
         W["upsample"] = ops.pack_conv(P["upsample.convtr.convtr.convtr.weight"].float(), None, cfg.dimension, dev)
-        def tlayers(root):
-            out = []
-            for li in range(cfg.num_layers):
-                L = f"{root}.transformer.layers.{li}"
-                out.append({
-                    "n1": (f(P[L + ".norm1.weight"]), f(P[L + ".norm1.bias"])), "n2": (f(P[L + ".norm2.weight"]), f(P[L + ".norm2.bias"])),
-                    "in_proj": ops.pack_linear(P[L + ".self_attn.in_proj.weight"].float(), None, dev),
-                    "out_proj": ops.pack_linear(P[L + ".self_attn.out_proj.weight"].float(), None, dev),
-                    "l1": ops.pack_linear(P[L + ".gating.linear1.weight"].float(), None, dev),
-                    "l2": ops.pack_linear(P[L + ".gating.linear2.weight"].float(), None, dev),
-                    "ls1": f(P[L + ".layer_scale_1.scale"]), "ls2": f(P[L + ".layer_scale_2.scale"])})
-            return out
-
         W["layers"] = []
         for li in range(cfg.num_layers):
             L = f"decoder_transformer.transformer.layers.{li}"
@@ -201,18 +188,7 @@ class Mimi:
         self._w = W
         self._enc = None
         if "encoder.init_conv1d.conv.conv.weight" in P:                 # encode side (seanet.py:194-199, mimi.py:146-153, quantization.py:178-185)
-            E = {"init": cw("encoder.init_conv1d.conv.conv"), "layers": [], "final": cw("encoder.final_conv1d.conv.conv"),
-                 "tr": tlayers("encoder_transformer"), "down": cw("downsample.conv.conv.conv")}
-            for li, r in enumerate(reversed(cfg.ratios)):
-                L = f"encoder.layers.{li}"
-                E["layers"].append({"r": r, "c0": cw(L + ".residuals.0.block.0.conv.conv"), "c1": cw(L + ".residuals.0.block.1.conv.conv"),
-                                    "down": cw(L + ".downsample.conv.conv")})
-            for name, cb in (("first", W["cb_first"]), ("rest", W["cb_rest"])):
-                if cb is None:
-                    continue
-                E["in_" + name] = ops.pack_conv(P[f"quantizer.rvq_{name}.input_proj.weight"].float(), None, 1, dev)
-                E["c2_" + name] = ((cb.double() ** 2).sum(-1) / 2).contiguous()             # |e|^2 / 2 of argmin(|e|^2 / 2 - x.e)
-            self._enc = E
+            self._enc = load_encoder(P, cfg, dev, W["cb_first"], W["cb_rest"])
         return self
 
     @torch.no_grad()
@@ -241,65 +217,114 @@ class Mimi:
         return pcm.reshape(B, 1, -1)
 
     def _transformer(self, x: torch.Tensor, layers) -> torch.Tensor:
-        """ProjectedTransformer (mimi/modules/transformer.py:63-261), fresh cache: pre-norm layers, traditional RoPE, causal attention
-        inside a ``context``-position window, LayerScale on both residual branches."""
-        cfg = self.cfg
-        d, nh = cfg.dimension, cfg.num_heads
-        for lw in layers:
-            n1 = ops.layernorm(x, *lw["n1"], eps=1e-5)
-            qkv = ops.linear(n1, lw["in_proj"])
-            ops.rope_(qkv[:, :, :d], nh, offset=0, base=cfg.max_period, traditional=True)
-            ops.rope_(qkv[:, :, d:2 * d], nh, offset=0, base=cfg.max_period, traditional=True)
-            att = ops.attention(qkv[:, :, :d], qkv[:, :, d:2 * d], qkv[:, :, 2 * d:], n_heads=nh, scale=(d // nh) ** -0.5,
-                                causal=True, window=cfg.context)
-            x = ops.linear(att, lw["out_proj"], cscale=lw["ls1"], res=x)
-            n2 = ops.layernorm(x, *lw["n2"], eps=1e-5)
-            m = ops.linear(n2, lw["l1"], post_act=ACT["gelu_tanh"])
-            x = ops.linear(m, lw["l2"], cscale=lw["ls2"], res=x)
-        return x
-
-    @staticmethod
-    def _cconv(x, cw, ksize, stride=1, pre=None, pad_mode=0, res=None):
-        """StreamableConv1d (mimi/modules/conv.py:224-243), causal: k - stride samples of left padding, the right edge padded up to a whole
-        last frame (zeros, or the edge sample for ``pad_mode=1``)."""
-        L = x.shape[1]
-        pad_total = ksize - stride
-        lout = int(math.ceil(max(L + pad_total - ksize, 0) / stride + 1.0))
-        return ops.conv1d(x, cw, stride=stride, pad_left=pad_total, lout=lout, pad_mode=pad_mode, pre=pre, res=res)
+        return _transformer(x, layers, self.cfg)
 
     @torch.no_grad()
     def encode_latent(self, xs: torch.Tensor) -> torch.Tensor:
         """pcm [B, 1, n] -> the 12.5 Hz latent [B, ceil(n / 1920), 512] in front of the quantiser (mimi.py:146-152)."""
         if self._enc is None:
             raise ValueError("Mimi.encode: the loaded weights have no encoder (encoder.*, encoder_transformer.*, downsample.*)")
-        E, cfg = self._enc, self.cfg
-        x = xs.to(device=self.device, dtype=torch.float32)
-        x = x.reshape(x.shape[0], -1, 1)                                 # [B, 1, n] -> [B, n, 1] (one channel: same memory)
-        elu = Pre(act=ACT["elu"])
-        x = self._cconv(x, E["init"], cfg.ksize)
-        for lw in E["layers"]:
-            t = self._cconv(x, lw["c0"], cfg.residual_ksize, pre=elu)
-            y = self._cconv(t, lw["c1"], 1, pre=elu, res=x)               # block(x) + x  (seanet.py:61-66)
-            x = self._cconv(y, lw["down"], 2 * lw["r"], stride=lw["r"], pre=elu)
-        x = self._cconv(x, E["final"], cfg.last_ksize, pre=elu)
-        x = self._transformer(x, E["tr"])
-        s = cfg.upsample_stride
-        return self._cconv(x, E["down"], 2 * s, stride=s, pad_mode=1)
+        return encode_latent(self._enc, self.cfg, xs, self.device)
 
     @torch.no_grad()
     def encode(self, xs: torch.Tensor) -> torch.Tensor:
         """mimi.py:146-153: pcm [B, 1, n] -> int64 codes [B, nq, ceil(n / 1920)]: SEANet encoder, encoder transformer, stride-2 replicate-padded
         down-sampling conv, then the split residual quantiser (quantization.py:178-185): the first codebook on its own projection, the other
         nq - 1 as a residual chain on theirs -- `rvq_encode_kernel` runs the chain (argmin |e|^2 / 2 - x.e, first index on ties)."""
-        z = self.encode_latent(xs)
-        E, W = self._enc, self._w
-        B, T, _ = z.shape
-        r1 = ops.conv1d(z, E["in_first"])
-        codes = [ops.rvq_encode(r1.reshape(B * T, -1), W["cb_first"], E["c2_first"]).reshape(B, T, 1)]
-        if W["cb_rest"] is not None:
-            r2 = ops.conv1d(z, E["in_rest"])
-            codes.append(ops.rvq_encode(r2.reshape(B * T, -1), W["cb_rest"], E["c2_rest"]).reshape(B, T, -1))
-        return torch.cat(codes, dim=2).transpose(1, 2).contiguous()
+        return encode_codes(self._enc, self.encode_latent(xs))
+
+
+# ------------------------------------------------------------------------------------------------------------------- encode side
+# Shared by Mimi.encode and the Qwen3-TTS speech-tokenizer encoder (speech_tokenizer.py:957-1058), which is Mimi's encoder with a full
+# causal mask, half-split RoPE and only its first code books kept.
+def _transformer(x: torch.Tensor, layers, cfg: MimiConfig, rope_traditional: bool = True, window=None) -> torch.Tensor:
+    """ProjectedTransformer (mimi/modules/transformer.py:63-261), fresh cache: pre-norm layers, RoPE (``rope_traditional``: interleaved
+    pairs, else rotate_half), causal attention inside a ``window``-position window (None: ``cfg.context``; 0: full causal), LayerScale on
+    both residual branches."""
+    d, nh = cfg.dimension, cfg.num_heads
+    win = cfg.context if window is None else window
+    for lw in layers:
+        n1 = ops.layernorm(x, *lw["n1"], eps=1e-5)
+        qkv = ops.linear(n1, lw["in_proj"])
+        ops.rope_(qkv[:, :, :d], nh, offset=0, base=cfg.max_period, traditional=rope_traditional)
+        ops.rope_(qkv[:, :, d:2 * d], nh, offset=0, base=cfg.max_period, traditional=rope_traditional)
+        att = ops.attention(qkv[:, :, :d], qkv[:, :, d:2 * d], qkv[:, :, 2 * d:], n_heads=nh, scale=(d // nh) ** -0.5,
+                            causal=True, window=win)
+        x = ops.linear(att, lw["out_proj"], cscale=lw["ls1"], res=x)
+        n2 = ops.layernorm(x, *lw["n2"], eps=1e-5)
+        m = ops.linear(n2, lw["l1"], post_act=ACT["gelu_tanh"])
+        x = ops.linear(m, lw["l2"], cscale=lw["ls2"], res=x)
+    return x
+
+
+def _cconv(x, cw, ksize, stride=1, pre=None, pad_mode=0, res=None):
+    """StreamableConv1d (mimi/modules/conv.py:224-243), causal: k - stride samples of left padding, the right edge padded up to a whole
+    last frame (zeros, or the edge sample for ``pad_mode=1``)."""
+    L = x.shape[1]
+    pad_total = ksize - stride
+    lout = int(math.ceil(max(L + pad_total - ksize, 0) / stride + 1.0))
+    return ops.conv1d(x, cw, stride=stride, pad_left=pad_total, lout=lout, pad_mode=pad_mode, pre=pre, res=res)
+
+
+def load_encoder(P, cfg: MimiConfig, dev, cb_first: torch.Tensor, cb_rest) -> dict:
+    """Encode-side weights from the reference's names (``encoder.*``, ``encoder_transformer.*``, ``downsample.*``, the quantiser's
+    ``input_proj``s) and the quantiser's codebooks ``cb_first`` [1, bins, qdim] / ``cb_rest`` [nq - 1, bins, qdim] (or None)."""
+    f = lambda t: t.float().to(dev).contiguous()
+    cw = lambda pre: ops.pack_conv(P[pre + ".weight"].float(), P.get(pre + ".bias"), 1, dev)
+    tr = []
+    for li in range(cfg.num_layers):
+        L = f"encoder_transformer.transformer.layers.{li}"
+        tr.append({
+            "n1": (f(P[L + ".norm1.weight"]), f(P[L + ".norm1.bias"])), "n2": (f(P[L + ".norm2.weight"]), f(P[L + ".norm2.bias"])),
+            "in_proj": ops.pack_linear(P[L + ".self_attn.in_proj.weight"].float(), None, dev),
+            "out_proj": ops.pack_linear(P[L + ".self_attn.out_proj.weight"].float(), None, dev),
+            "l1": ops.pack_linear(P[L + ".gating.linear1.weight"].float(), None, dev),
+            "l2": ops.pack_linear(P[L + ".gating.linear2.weight"].float(), None, dev),
+            "ls1": f(P[L + ".layer_scale_1.scale"]), "ls2": f(P[L + ".layer_scale_2.scale"])})
+    E = {"init": cw("encoder.init_conv1d.conv.conv"), "layers": [], "final": cw("encoder.final_conv1d.conv.conv"), "tr": tr,
+         "down": cw("downsample.conv.conv.conv"), "cb_first": cb_first, "cb_rest": cb_rest}
+    for li, r in enumerate(reversed(cfg.ratios)):
+        L = f"encoder.layers.{li}"
+        E["layers"].append({"r": r, "c0": cw(L + ".residuals.0.block.0.conv.conv"), "c1": cw(L + ".residuals.0.block.1.conv.conv"),
+                            "down": cw(L + ".downsample.conv.conv")})
+    for name, cb in (("first", cb_first), ("rest", cb_rest)):
+        if cb is None:
+            continue
+        E["in_" + name] = ops.pack_conv(P[f"quantizer.rvq_{name}.input_proj.weight"].float(), None, 1, dev)
+        E["c2_" + name] = ((cb.double() ** 2).sum(-1) / 2).contiguous()             # |e|^2 / 2 of argmin(|e|^2 / 2 - x.e)
+    return E
+
+
+def encode_latent(E: dict, cfg: MimiConfig, xs: torch.Tensor, device, *, rope_traditional: bool = True, window=None) -> torch.Tensor:
+    """pcm [B, 1, n] -> latent [B, ceil(n / 1920), dimension]: SEANet encoder, encoder transformer (switches as in ``_transformer``),
+    stride-2 replicate-padded down-sampling conv."""
+    x = xs.to(device=device, dtype=torch.float32)
+    x = x.reshape(x.shape[0], -1, 1)                                 # [B, 1, n] -> [B, n, 1] (one channel: same memory)
+    elu = Pre(act=ACT["elu"])
+    x = _cconv(x, E["init"], cfg.ksize)
+    for lw in E["layers"]:
+        t = _cconv(x, lw["c0"], cfg.residual_ksize, pre=elu)
+        y = _cconv(t, lw["c1"], 1, pre=elu, res=x)                   # block(x) + x  (seanet.py:61-66)
+        x = _cconv(y, lw["down"], 2 * lw["r"], stride=lw["r"], pre=elu)
+    x = _cconv(x, E["final"], cfg.last_ksize, pre=elu)
+    x = _transformer(x, E["tr"], cfg, rope_traditional, window)
+    s = cfg.upsample_stride
+    return _cconv(x, E["down"], 2 * s, stride=s, pad_mode=1)
+
+
+def encode_codes(E: dict, z: torch.Tensor, n_books=None) -> torch.Tensor:
+    """Split residual quantiser (quantization.py:178-185): latent [B, T, dimension] -> int64 codes [B, n_books, T] (default: every book).
+    The residual chain is sequential, so running only the first ``n_books`` gives exactly the first ``n_books`` codes of the full chain."""
+    B, T, _ = z.shape
+    r1 = ops.conv1d(z, E["in_first"])
+    codes = [ops.rvq_encode(r1.reshape(B * T, -1), E["cb_first"], E["c2_first"]).reshape(B, T, 1)]
+    n_rest = 0 if E["cb_rest"] is None else E["cb_rest"].shape[0]
+    if n_books is not None:
+        n_rest = min(n_rest, n_books - 1)
+    if n_rest > 0:
+        r2 = ops.conv1d(z, E["in_rest"])
+        codes.append(ops.rvq_encode(r2.reshape(B * T, -1), E["cb_rest"][:n_rest], E["c2_rest"][:n_rest]).reshape(B, T, -1))
+    return torch.cat(codes, dim=2).transpose(1, 2).contiguous()
 
 
 class MimiStreamingDecoder:

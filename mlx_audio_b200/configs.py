@@ -49,3 +49,9 @@ QWEN3_TOKENIZER_DECODER = {
     "num_hidden_layers": 8, "num_key_value_heads": 16, "num_quantizers": 16, "num_semantic_quantizers": 1,
     "rms_norm_eps": 1e-5, "rope_theta": 10000.0, "upsample_rates": [8, 5, 4, 3], "upsampling_ratios": [2, 2],
 }
+
+QWEN3_TOKENIZER_ENCODER = {      # the speech-tokenizer encoder (ICL voice cloning) in Mimi's vocabulary: synth.qwen3_tokenizer_weights(encoder=)
+    "dimension": 512, "nfilters": 64, "ratios": [8, 6, 5, 4], "ksize": 7, "residual_ksize": 3, "last_ksize": 3, "compress": 2, "d_model": 512,
+    "num_heads": 8, "num_layers": 8, "dim_feedforward": 2048, "context": 250, "max_period": 10000, "layer_scale": 0.01, "nq": 32, "bins": 2048,
+    "qdim": 256, "upsample_stride": 2, "valid_num_quantizers": 16,
+}

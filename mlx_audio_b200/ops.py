@@ -975,6 +975,21 @@ def attn_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, n
     return out
 
 
+def attn_prefill(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, *, scale: float,
+                 base_dev=None, base: int = 0, kv_start=None, max_k: Optional[int] = None, out=None) -> torch.Tensor:
+    """``attn_decode``'s contract on the tensor cores, for prefills of >= 64 rows with head_dim 128 and two query heads per KV head."""
+    _chk3(q, "q")
+    B, S, _ = q.shape
+    if out is None:
+        out = torch.empty(B, S, n_heads * head_dim, device=q.device, dtype=torch.float32)
+    if max_k is None:
+        max_k = k_cache.shape[1] if base_dev is not None else base + S
+    _call("attention", _lib.lib().b2a_attn_prefill, 1, q.data_ptr(), q.stride(0), q.stride(1), k_cache.data_ptr(), v_cache.data_ptr(),
+          k_cache.stride(0), k_cache.stride(1), out.data_ptr(), out.stride(0), out.stride(1), B, S, n_heads, n_kv, head_dim, scale,
+          _p(base_dev), base, _p(kv_start), max_k, _stream())
+    return out
+
+
 def attn_decode_fused(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, k_cache: torch.Tensor, v_cache: torch.Tensor, *, scale: float,
                       q_norm=None, k_norm=None, eps: float = 1e-6, pos3=None, base_dev=None, base: int = 0, mrope=(0, 0),
                       theta: float = 10000.0, kv_start=None, out=None) -> torch.Tensor:

@@ -455,9 +455,11 @@ def qwen3_talker_weights(cfg, text_vocab=512, seed=11):
     return g.P
 
 
-def qwen3_tokenizer_weights(cfg, seed=12):
+def qwen3_tokenizer_weights(cfg, seed=12, encoder=None):
     """Parameter tree of speech_tokenizer.py:Qwen3TTSSpeechTokenizer (decode side, MLX names after ``sanitize``); ``cfg`` is the
-    flat dict of oracle/qwen3.py:TOKENIZER_DECODER.  bf16-exact values."""
+    flat dict of oracle/qwen3.py:TOKENIZER_DECODER.  bf16-exact values.  ``encoder`` = the flat dict of oracle/qwen3.py:TOKENIZER_ENCODER
+    adds the speech-tokenizer encoder (``encoder_model.*``, the names of Qwen3TTSSpeechTokenizerEncoder.sanitize): Mimi's encode side at
+    those shapes, drawn from its own stream (the decoder's tensors keep their values)."""
     g = _Gen(seed)
     gen = g.g
     cd, ld, hs = cfg["codebook_dim"], cfg["latent_dim"], cfg["hidden_size"]
@@ -527,6 +529,9 @@ def qwen3_tokenizer_weights(cfg, seed=12):
     g.P[f"{D}decoder.{n_blocks + 1}.beta"] = _bf16(0.2 * torch.randn(cin, generator=gen))
     _fan(g, f"{D}decoder.{n_blocks + 2}.conv.weight", 1, 7, cin, fan_in=7 * cin * 16)
     g.normal(f"{D}decoder.{n_blocks + 2}.conv.bias", 1, std=0.02)
+    if encoder is not None:
+        keep = ("encoder.", "encoder_transformer.", "downsample.", "quantizer.")
+        g.P.update({"encoder_model." + k: v for k, v in mimi_weights(encoder, seed=seed + 1, encoder=True).items() if k.startswith(keep)})
     return g.P
 
 

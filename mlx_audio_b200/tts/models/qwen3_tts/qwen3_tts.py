@@ -2,7 +2,10 @@
 
 Covers the base path of ``Model.generate`` (qwen3_tts.py:1122-1575): input assembly from token ids
 (``_prepare_generation_inputs`` :326-484 after the host tokenizer, with x-vector cloning through ``speaker_encoder.py``), the per-frame
-loop (:1323-1404) with ``_sample_token`` (:805-860), and ``_decode_chunk`` (:1017-1048) through the speech tokenizer.
+loop (:1323-1404) with ``_sample_token`` (:805-860), and ``_decode_chunk`` (:1017-1048) through the speech tokenizer; and in-context
+voice cloning from reference audio + its transcript (``_generate_icl`` :2200-2510): the speech-tokenizer encoder turns the reference into
+codes, one prompt row per reference frame (``_prepare_icl_generation_inputs`` :606-803), the same frame loop, and a joint decode of
+[reference | generated] codes with the reference's share cut off (``_decode_icl_generated_codes`` :1085-1112).
 
 One frame = talker step + first-codebook sample + 15 code-predictor sub-steps (each with its sampler) + next-input
 embedding sum: ~700 small launches.  They are captured ONCE into a CUDA graph; every scalar that changes between frames
@@ -76,6 +79,7 @@ class Model:
         self.supported_speakers = list(tc.spk_id.keys()) if tc.spk_id else []
         self.supported_languages = ["auto"] + [l for l in (tc.codec_language_id or {}) if "dialect" not in l]
         self._graph = None
+        self._icl_cache = {}        # (ref_text, (ref_audio size, ref_audio sum)) -> (ref codes [1, 16, T], ref ids) (qwen3_tts.py:639-664)
 
     def get_supported_speakers(self):
         return self.supported_speakers
@@ -135,7 +139,8 @@ class Model:
         """qwen3_tts.py:2818-2911: HF tokenizer (when its files are present), ``speech_tokenizer/`` sub-model, generation config."""
         import json
         from pathlib import Path
-        from .config import Qwen3TTSTokenizerConfig, Qwen3TTSTokenizerDecoderConfig, filter_dict_for_dataclass
+        from .config import Qwen3TTSTokenizerConfig, Qwen3TTSTokenizerDecoderConfig, Qwen3TTSTokenizerEncoderConfig, filter_dict_for_dataclass
+        from .speech_tokenizer import Qwen3TTSSpeechTokenizerEncoder
         model_path = Path(model_path)
         try:
             from transformers import AutoTokenizer
@@ -149,7 +154,9 @@ class Model:
             model.speech_tokenizer_has_encoder = "encoder_config" in d       # speech_tokenizer.py:1076-1097, read at qwen3_tts.py:2838-2854
             dec = Qwen3TTSTokenizerDecoderConfig(**filter_dict_for_dataclass(Qwen3TTSTokenizerDecoderConfig, d["decoder_config"])) \
                 if "decoder_config" in d else None
-            tc = Qwen3TTSTokenizerConfig(decoder_config=dec)
+            enc = Qwen3TTSTokenizerEncoderConfig(**filter_dict_for_dataclass(Qwen3TTSTokenizerEncoderConfig, d["encoder_config"])) \
+                if "encoder_config" in d else None
+            tc = Qwen3TTSTokenizerConfig(decoder_config=dec, encoder_config=enc)
             for k, v in d.items():
                 if k not in ("decoder_config", "encoder_config") and hasattr(tc, k):
                     setattr(tc, k, v)
@@ -157,7 +164,8 @@ class Model:
             for wf in sorted(st_path.glob("*.safetensors")):
                 w.update(load_file(str(wf)))
             if w:
-                st = Qwen3TTSSpeechTokenizer(tc, model.device).load_weights(Qwen3TTSSpeechTokenizer.sanitize(w))
+                st = Qwen3TTSSpeechTokenizer(tc, model.device).load_weights({**Qwen3TTSSpeechTokenizer.sanitize(w),
+                                                                             **Qwen3TTSSpeechTokenizerEncoder.sanitize(w)})
                 model.load_speech_tokenizer(st)
         gen = model_path / "generation_config.json"
         if gen.exists():
@@ -173,9 +181,31 @@ class Model:
         t, cfg, dev = self.talker, self.config.talker_config, self.device
         ids = torch.as_tensor(input_ids, dtype=torch.int64, device=dev).reshape(-1)
         text_embed = t.text_projection(ops.gather_rows(t.text_embedding, ids)[None])                          # [1,L,H]
+        tts_bos, tts_eos, tts_pad = self._tts_embeds()
+        combined = self._codec_prefix(language_id, speaker_id, speaker_embed, tts_pad, tts_bos)
+        first_text = text_embed[:, 3:4] + self._codec_rows([cfg.codec_bos_id])
+        parts = [text_embed[:, :3], combined, first_text]
+        if instruct_ids is not None:                                      # "<|im_start|>user\n{instruct}<|im_end|>\n" (:452-458,473-476)
+            iid = torch.as_tensor(instruct_ids, dtype=torch.int64, device=dev).reshape(-1)
+            parts = [t.text_projection(ops.gather_rows(t.text_embedding, iid)[None])] + parts
+        input_embeds = torch.cat(parts, dim=1).contiguous()
+        trailing = torch.cat([text_embed[:, 4:-5], tts_eos], dim=1).contiguous()
+        return input_embeds, trailing, tts_pad.contiguous()
+
+    def _tts_embeds(self):
+        """Projected (tts_bos, tts_eos, tts_pad) text embeddings, each [1, 1, H]."""
+        t, dev = self.talker, self.device
         tts_ids = torch.tensor([self.config.tts_bos_token_id, self.config.tts_eos_token_id, self.config.tts_pad_token_id], device=dev)
         tts = t.text_projection(ops.gather_rows(t.text_embedding, tts_ids)[None])
-        tts_bos, tts_eos, tts_pad = tts[:, 0:1], tts[:, 1:2], tts[:, 2:3]
+        return tts[:, 0:1], tts[:, 1:2], tts[:, 2:3]
+
+    def _codec_rows(self, ids) -> torch.Tensor:
+        return ops.gather_rows(self.talker.codec_embedding, torch.tensor(ids, device=self.device))[None]
+
+    def _codec_prefix(self, language_id, speaker_id, speaker_embed, tts_pad, tts_bos) -> torch.Tensor:
+        """The rows between the role and the text (qwen3_tts.py:416-450, 748-796): think / language ids, speaker row, pad, overlaid with
+        tts_pad ... tts_bos on the text side.  [1, n, H]"""
+        t, cfg, dev = self.talker, self.config.talker_config, self.device
         if speaker_embed is None and speaker_id is not None:
             speaker_embed = ops.gather_rows(t.codec_embedding, torch.tensor([int(speaker_id)], device=dev))[None]
         elif speaker_embed is not None and self.talker_dtype != torch.float32:
@@ -185,20 +215,41 @@ class Model:
             prefill = [cfg.codec_nothink_id, cfg.codec_think_bos_id, cfg.codec_think_eos_id]
         else:
             prefill = [cfg.codec_think_id, cfg.codec_think_bos_id, int(language_id), cfg.codec_think_eos_id]
-        codec = ops.gather_rows(t.codec_embedding, torch.tensor(prefill, device=dev))[None]
-        suffix = ops.gather_rows(t.codec_embedding, torch.tensor([cfg.codec_pad_id, cfg.codec_bos_id], device=dev))[None]
+        codec = self._codec_rows(prefill)
+        suffix = self._codec_rows([cfg.codec_pad_id])
         parts = [codec] + ([speaker_embed.reshape(1, 1, -1).float()] if speaker_embed is not None else []) + [suffix]
         codec = torch.cat(parts, dim=1)
-        role = text_embed[:, :3]
-        combined = torch.cat([tts_pad.expand(1, codec.shape[1] - 2, -1), tts_bos], dim=1) + codec[:, :-1]
-        first_text = text_embed[:, 3:4] + codec[:, -1:]
-        parts = [role, combined, first_text]
-        if instruct_ids is not None:                                      # "<|im_start|>user\n{instruct}<|im_end|>\n" (:452-458,473-476)
-            iid = torch.as_tensor(instruct_ids, dtype=torch.int64, device=dev).reshape(-1)
-            parts = [t.text_projection(ops.gather_rows(t.text_embedding, iid)[None])] + parts
-        input_embeds = torch.cat(parts, dim=1).contiguous()
-        trailing = torch.cat([text_embed[:, 4:-5], tts_eos], dim=1).contiguous()
-        return input_embeds, trailing, tts_pad.contiguous()
+        return torch.cat([tts_pad.expand(1, codec.shape[1] - 1, -1), tts_bos], dim=1) + codec
+
+    @torch.no_grad()
+    def prepare_icl_generation_inputs_from_ids(self, target_ids, ref_ids, ref_codes, language_id: Optional[int] = None, speaker_embed=None):
+        """_prepare_icl_generation_inputs (qwen3_tts.py:606-803) after tokenisation and reference encoding.  ``target_ids`` = ids of
+        "<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n", ``ref_ids`` = ids of "<|im_start|>assistant\n{ref_text}<|im_end|>\n",
+        ``ref_codes`` [1, 16, T_ref] from the speech-tokenizer encoder, ``speaker_embed`` [1, H] (x-vector) or None.  Prompt = role,
+        codec prefix, then every text row (reference transcript + target text + tts_eos, each + codec_pad), then the codec-bos row and one
+        row per reference frame (tts_pad + sum_g table_g[code_g]).  Returns (input_embeds [1, P, H], trailing = tts_pad, tts_pad)."""
+        t, cfg, dev = self.talker, self.config.talker_config, self.device
+        target = torch.as_tensor(target_ids, dtype=torch.int64, device=dev).reshape(-1)
+        ref = torch.as_tensor(ref_ids, dtype=torch.int64, device=dev).reshape(-1)
+        tts_bos, tts_eos, tts_pad = self._tts_embeds()
+        text = t.text_projection(ops.gather_rows(t.text_embedding, torch.cat([ref[3:-2], target[3:-5]]))[None])
+        text = torch.cat([text, tts_eos], dim=1) + self._codec_rows([cfg.codec_pad_id])
+        codes = torch.as_tensor(ref_codes, dtype=torch.int64).to(dev)[0].transpose(0, 1).contiguous()        # [T_ref, 16]
+        ref_rows = ops.embed_sum(codes, self._tabs_all, pad=tts_pad.reshape(-1).contiguous())[None]          # tts_pad + sum_g table_g[code_g]
+        bos = self._codec_rows([cfg.codec_bos_id]) + tts_pad
+        role = t.text_projection(ops.gather_rows(t.text_embedding, target[:3])[None])
+        combined = self._codec_prefix(language_id, None, speaker_embed, tts_pad, tts_bos)
+        input_embeds = torch.cat([role, combined, text, bos, ref_rows], dim=1).contiguous()
+        return input_embeds, tts_pad.contiguous(), tts_pad.contiguous()
+
+    @torch.no_grad()
+    def encode_reference(self, ref_audio) -> torch.Tensor:
+        """24 kHz reference samples [n] (or [1, n], [1, 1, n]) -> its codes [1, 16, ceil(n / 1920)] (qwen3_tts.py:644-652)."""
+        if self.speech_tokenizer is None or not self.speech_tokenizer.has_encoder:
+            raise NotImplementedError("in-context (ICL) voice cloning needs the speech tokenizer's encoder weights, which are not loaded; "
+                                      "pass ref_audio without ref_text for x-vector cloning")
+        a = ref_audio if isinstance(ref_audio, torch.Tensor) else torch.as_tensor(ref_audio)
+        return self.speech_tokenizer.encode(a.to(self.device).float().reshape(1, 1, -1))
 
     def extract_speaker_embedding(self, audio, sr: int = 24000) -> torch.Tensor:
         """qwen3_tts.py:285-324: 24 kHz samples [n] or [B, n] -> x-vector [B, enc_dim] (float32): log-mel front end + ECAPA-TDNN."""
@@ -564,6 +615,75 @@ class Model:
                                audio_samples={"samples": samples, "samples-per-sec": round(samples / dt, 2) if dt > 0 else 0},
                                processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
 
+    def generate_icl_from_ids(self, target_ids, ref_ids, *, ref_audio=None, ref_codes=None, speaker_embed=None, language_id=None,
+                              temperature: float = 0.9, max_tokens: int = 4096, top_k: int = 50, top_p: float = 1.0,
+                              repetition_penalty: float = 1.5, seed: int = 0, u=None, stream: bool = False, streaming_interval: float = 2.0,
+                              **kwargs):
+        """``_generate_icl`` (qwen3_tts.py:2200-2510) for already-tokenised texts (ids as in ``prepare_icl_generation_inputs_from_ids``).
+        ``ref_codes`` [1, 16, T_ref] are the reference's codes, or encoded here from ``ref_audio``; the x-vector of ``ref_audio`` takes the
+        speaker row (``speaker_embed`` [1, H] instead pins it).  Yields one GenerationResult: [ref | generated] codes decoded together,
+        trimmed to the valid length and with the reference's proportional share cut off; or with ``stream=True`` one chunk per
+        ``streaming_interval`` seconds of generated frames (segment 0, generated codes only)."""
+        if self.speech_tokenizer is None:
+            raise ValueError("Speech tokenizer not loaded")
+        t0 = time.perf_counter()
+        if ref_codes is None:
+            if ref_audio is None:
+                raise ValueError("generate_icl_from_ids: pass ref_audio or ref_codes")
+            ref_codes = self.encode_reference(ref_audio)
+        if speaker_embed is None and ref_audio is not None and self.speaker_encoder is not None:
+            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        x, trailing, pad = self.prepare_icl_generation_inputs_from_ids(target_ids, ref_ids, ref_codes, language_id, speaker_embed)
+        gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u)
+        if stream:
+            yield from self._stream_segment(x, trailing, pad, 0, streaming_interval, gen)
+            return
+        codes = self.generate_codes(x, trailing, pad, **gen)
+        if codes.shape[1] == 0:
+            return
+        audio = self._decode_icl_generated_codes(codes[0], ref_codes)
+        torch.cuda.synchronize(self.device)
+        dt = time.perf_counter() - t0
+        samples, n = int(audio.shape[0]), int(codes.shape[1])
+        dur = samples / self.sample_rate
+        yield GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=0, token_count=n,
+                               audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0.0,
+                               prompt={"tokens": n, "tokens-per-sec": n / dt if dt > 0 else 0},
+                               audio_samples={"samples": samples, "samples-per-sec": samples / dt if dt > 0 else 0},
+                               processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+
+    @torch.no_grad()
+    def _decode_icl_generated_codes(self, gen_codes: torch.Tensor, ref_codes: torch.Tensor) -> torch.Tensor:
+        """qwen3_tts.py:1085-1112: gen_codes [n, 16] -> the target's audio: [ref | generated] decoded together, trimmed to the valid length
+        (frames whose first code is > 0), then int(T_ref / total * samples) samples of reference cut off the front."""
+        ref_t = torch.as_tensor(ref_codes, dtype=torch.int64).to(self.device)[0].transpose(0, 1)
+        full = torch.cat([ref_t, gen_codes.to(self.device)], dim=0)[None]
+        wav, lengths = self.speech_tokenizer.decode(full)
+        audio = wav[0]
+        valid = int(lengths[0])
+        if 0 < valid < audio.shape[0]:
+            audio = audio[:valid]
+        cut = int(ref_t.shape[0] / max(full.shape[1], 1) * audio.shape[0])
+        return audio[cut:] if 0 < cut < audio.shape[0] else audio
+
+    def _generate_icl(self, text, ref_audio, ref_text, language, stream, streaming_interval, **gen):
+        """_generate_icl (qwen3_tts.py:2200-2510): the text is one segment; the reference's codes (and transcript ids) are cached on
+        (ref_text, (size, sum) of ref_audio), so a repeated reference does not run the encoder again (:639-664)."""
+        if self.tokenizer is None:
+            raise ValueError("Tokenizer not loaded. Call post_load_hook first.")
+        cfg = self.config.talker_config
+        a = ref_audio if isinstance(ref_audio, torch.Tensor) else torch.as_tensor(ref_audio)
+        key = (ref_text, (int(a.numel()), float(a.sum())))
+        if key not in self._icl_cache:
+            self._icl_cache[key] = (self.encode_reference(a), self.tokenizer.encode(f"<|im_start|>assistant\n{ref_text}<|im_end|>\n"))
+        ref_codes, ref_ids = self._icl_cache[key]
+        target_ids = self.tokenizer.encode(f"<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n")
+        language_id = None
+        if language.lower() != "auto" and cfg.codec_language_id and language.lower() in cfg.codec_language_id:
+            language_id = cfg.codec_language_id[language.lower()]
+        yield from self.generate_icl_from_ids(target_ids, ref_ids, ref_audio=a, ref_codes=ref_codes, language_id=language_id, stream=stream,
+                                              streaming_interval=streaming_interval, **gen)
+
     def _generate_segments(self, text, split_pattern, speaker, language, instruct, stream=False, streaming_interval=2.0, ref_audio=None, **gen):
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
@@ -614,11 +734,12 @@ class Model:
             return
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
-        if ref_audio is not None and ref_text is not None and self.speech_tokenizer_has_encoder:
-            # in-context cloning (_generate_icl, qwen3_tts.py:1233-1256): needs the speech-tokenizer encoder, which has no CUDA path yet --
-            # refuse instead of silently synthesising another voice
-            raise NotImplementedError("in-context (ICL) voice cloning from ref_audio + ref_text is not implemented; pass ref_audio "
-                                      "without ref_text for x-vector cloning")
+        if ref_audio is not None and ref_text is not None and (self.speech_tokenizer_has_encoder or self.speech_tokenizer.has_encoder):
+            # in-context cloning (qwen3_tts.py:1227-1252) with a stronger repetition penalty; a checkpoint that declares an encoder whose
+            # weights are missing raises (encode_reference) instead of silently synthesising another voice
+            gen["repetition_penalty"] = max(repetition_penalty, 1.5)
+            yield from self._generate_icl(text, ref_audio, ref_text, lang_code, stream, streaming_interval, **gen)
+            return
         if voice is not None and voice.lower() not in [s.lower() for s in self.supported_speakers]:
             raise ValueError(f"Voice '{voice}' is not supported by this Base model. Base models have no built-in preset voices — "
                              "clone a voice by passing ref_audio and ref_text instead.")

@@ -1,8 +1,10 @@
-"""Qwen3-TTS 12.5 Hz speech tokenizer, decode side, on H100 (reference: tts/models/qwen3_tts/speech_tokenizer.py).
+"""Qwen3-TTS 12.5 Hz speech tokenizer on H100 (reference: tts/models/qwen3_tts/speech_tokenizer.py).
 
 ``Qwen3TTSSpeechTokenizer(cfg).load_weights(...)``; ``decode(audio_codes[B,T,16]) -> (wav[B,samples], lengths)``
 (speech_tokenizer.py:1099-1118), ``batch_decode`` (:1120-1179), ``streaming_decode`` (:1181-1217) and the decoder's
-``__call__`` / ``chunked_decode`` (:843-880, 932-954) and the incremental ``streaming_step`` / ``reset_streaming_state`` (:882-930).
+``__call__`` / ``chunked_decode`` (:843-880, 932-954) and the incremental ``streaming_step`` / ``reset_streaming_state`` (:882-930).  ``encode(audio[B,1,n]) -> codes[B,16,ceil(n/1920)]``
+(:1082-1093) through ``Qwen3TTSSpeechTokenizerEncoder`` (:957-1058) when the checkpoint has encoder weights: Mimi's encode chain
+(codec/models/mimi.py), with a full causal mask and half-split RoPE in its transformer.
 
 H100 mapping: RVQ gather-sum in one kernel; every dense conv / linear runs on the wgmma conv kernel with the SnakeBeta /
 LayerScale / gamma / residual / clip fused as prologue or epilogue; the 300-frame chunks of ``chunked_decode`` are
@@ -16,8 +18,9 @@ import numpy as np
 import torch
 
 from .... import ops
+from ....codec.models import mimi
 from ....ops import ACT, Pre
-from .config import Qwen3TTSTokenizerConfig, Qwen3TTSTokenizerDecoderConfig
+from .config import Qwen3TTSTokenizerConfig, Qwen3TTSTokenizerDecoderConfig, Qwen3TTSTokenizerEncoderConfig
 
 
 def check_array_shape_qwen3(arr) -> bool:
@@ -323,8 +326,108 @@ class Qwen3TTSSpeechTokenizerDecoder:
         return wav.reshape(B, 1, -1)
 
 
+class Qwen3TTSSpeechTokenizerEncoder:
+    """speech_tokenizer.py:957-1058: SEANet encoder -> encoder transformer -> stride-2 ConvDownsample1d -> split RVQ, keeping the first
+    ``valid_num_quantizers`` code books.  The launch sequence is Mimi's encode (codec/models/mimi.py: ``encode_latent`` /
+    ``encode_codes``) with the two switches the reference sets here: a full causal mask (no ``context`` window, :1050-1055) and half-split
+    RoPE (``rope_traditional=False``, :1009).  The residual chain is sequential, so only the kept books are searched."""
+
+    def __init__(self, config: Qwen3TTSTokenizerEncoderConfig, valid_num_quantizers: int = 16, device="cuda"):
+        c = config
+        if c.num_key_value_heads != c.num_attention_heads or c.num_residual_layers != 1 or c.use_conv_shortcut or not c.use_causal_conv:
+            raise NotImplementedError("Qwen3TTSSpeechTokenizerEncoder: the encode chain covers causal convs, one identity-shortcut residual "
+                                      "layer per block and one KV head per attention head")
+        self.config = config
+        self.device = torch.device(device)
+        self.valid_num_quantizers = min(int(valid_num_quantizers), c.num_quantizers)
+        encoder_frame_rate = c.sampling_rate / float(np.prod(c.upsampling_ratios))
+        self.mimi_config = mimi.MimiConfig(
+            dimension=c.hidden_size, nfilters=c.num_filters, ratios=list(c.upsampling_ratios), ksize=c.kernel_size,
+            residual_ksize=c.residual_kernel_size, last_ksize=c.last_kernel_size, compress=c.compress, num_heads=c.num_attention_heads,
+            num_layers=c.num_hidden_layers, dim_feedforward=c.intermediate_size, context=c.sliding_window, max_period=float(int(c.rope_theta)),
+            nq=c.num_quantizers, bins=c.codebook_size, qdim=c.codebook_dim, upsample_stride=int(encoder_frame_rate / c.frame_rate),
+            sample_rate=float(c.sampling_rate), frame_rate=c.frame_rate)
+        self._enc = None
+
+    def load_weights(self, weights, prefix: str = "encoder_model."):
+        """``weights``: names and layouts of ``Qwen3TTSSpeechTokenizerEncoder.sanitize`` (``encoder_model.`` prefix), codebooks as
+        (embedding_sum, cluster_usage) -> embedding_sum / max(cluster_usage, 1e-5) (quantization.py:26-30)."""
+        P, cfg, dev = {k[len(prefix):]: v for k, v in dict(weights).items() if k.startswith(prefix)}, self.mimi_config, self.device
+
+        def emb(pre):
+            return P[pre + ".embedding_sum"].float() / torch.clamp(P[pre + ".cluster_usage"].float(), min=1e-5)[:, None]
+        cb_first = torch.stack([emb("quantizer.rvq_first.vq.layers.0.codebook")]).to(dev).contiguous()
+        cb_rest = torch.stack([emb(f"quantizer.rvq_rest.vq.layers.{i}.codebook") for i in range(cfg.nq - 1)]).to(dev).contiguous() \
+            if cfg.nq > 1 else None
+        self._enc = mimi.load_encoder(P, cfg, dev, cb_first, cb_rest)
+        return self
+
+    @torch.no_grad()
+    def encode_latent(self, audio: torch.Tensor) -> torch.Tensor:
+        """audio [B, 1, n] at 24 kHz -> the 12.5 Hz latent [B, ceil(n / 1920), hidden_size] in front of the quantiser."""
+        return mimi.encode_latent(self._enc, self.mimi_config, audio, self.device, rope_traditional=False, window=0)
+
+    @torch.no_grad()
+    def encode(self, audio: torch.Tensor) -> torch.Tensor:
+        """audio [B, 1, n] at 24 kHz -> int64 codes [B, valid_num_quantizers, ceil(n / 1920)] (:1037-1058)."""
+        return mimi.encode_codes(self._enc, self.encode_latent(audio), self.valid_num_quantizers)
+
+    @staticmethod
+    def sanitize(weights):
+        """Encoder half of speech_tokenizer.py:1220-1447: the checkpoint's ``encoder.*`` keys (transformers' Mimi state-dict names) ->
+        the reference's ``encoder_model.*`` module tree.  SEANet layer indices -> init / residual / downsample / final convs, q / k / v ->
+        one ``in_proj``, conv weights (out, in, K) -> (out, K, in), codebooks kept as (embedding_sum, cluster_usage)."""
+        conv_map = {0: "encoder.init_conv1d", 3: "encoder.layers.0.downsample", 6: "encoder.layers.1.downsample",
+                    9: "encoder.layers.2.downsample", 12: "encoder.layers.3.downsample", 14: "encoder.final_conv1d"}
+        res_map, blk_map = {1: 0, 4: 1, 7: 2, 10: 3}, {1: 0, 3: 1}
+        tr = {"self_attn.o_proj.weight": "self_attn.out_proj.weight", "mlp.fc1.weight": "gating.linear1.weight",
+              "mlp.fc2.weight": "gating.linear2.weight", "input_layernorm.weight": "norm1.weight", "input_layernorm.bias": "norm1.bias",
+              "post_attention_layernorm.weight": "norm2.weight", "post_attention_layernorm.bias": "norm2.bias",
+              "self_attn_layer_scale.scale": "layer_scale_1.scale", "mlp_layer_scale.scale": "layer_scale_2.scale"}
+        sw = lambda v: v.transpose(-1, -2) if v.dim() == 3 else v                                  # noqa: E731
+        out, qkv = {}, {}
+        for k, v in weights.items():
+            if not k.startswith("encoder."):
+                continue
+            v = torch.as_tensor(v)
+            parts = k.split(".")
+            if k.startswith("encoder.encoder.layers."):
+                n = int(parts[3])
+                if "block" in k:
+                    if n not in res_map or int(parts[5]) not in blk_map:
+                        continue
+                    base, suffix = f"encoder.layers.{res_map[n]}.residuals.0.block.{blk_map[int(parts[5])]}", ".".join(parts[6:])
+                else:
+                    if n not in conv_map:
+                        continue
+                    base, suffix = conv_map[n], ".".join(parts[4:])
+                out[f"encoder_model.{base}.conv.{suffix}"] = sw(v) if "weight" in suffix else v
+            elif k.startswith("encoder.encoder_transformer.layers."):
+                li, rest = int(parts[3]), ".".join(parts[4:])
+                if rest in ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight"):
+                    qkv.setdefault(li, {})[rest.split(".")[1][0]] = v
+                elif rest in tr:
+                    out[f"encoder_model.encoder_transformer.transformer.layers.{li}.{tr[rest]}"] = v
+            elif k.startswith("encoder.downsample."):
+                suffix = k[len("encoder.downsample."):]
+                out[f"encoder_model.downsample.conv.conv.{suffix}"] = sw(v) if "weight" in suffix else v
+            elif k.startswith("encoder.quantizer."):
+                rest = k[len("encoder.quantizer."):]
+                which = "rvq_first" if "semantic_residual_vector_quantizer" in rest else "rvq_rest"
+                if ".codebook.cluster_usage" in rest or ".codebook.embed_sum" in rest:
+                    li = int(rest.split("layers.")[1].split(".")[0])
+                    name = "cluster_usage" if "cluster_usage" in rest else "embedding_sum"
+                    out[f"encoder_model.quantizer.{which}.vq.layers.{li}.codebook.{name}"] = v
+                elif "input_proj.weight" in rest or "output_proj.weight" in rest:
+                    out[f"encoder_model.quantizer.{which}.{'input_proj' if 'input_proj' in rest else 'output_proj'}.weight"] = sw(v)
+        for li, d in qkv.items():
+            if len(d) == 3:
+                out[f"encoder_model.encoder_transformer.transformer.layers.{li}.self_attn.in_proj.weight"] = torch.cat([d["q"], d["k"], d["v"]], 0)
+        return out
+
+
 class Qwen3TTSSpeechTokenizer:
-    """speech_tokenizer.py:1061-1217 (decode side)."""
+    """speech_tokenizer.py:1061-1217."""
 
     def __init__(self, config: Qwen3TTSTokenizerConfig, device="cuda"):
         self.config = config
@@ -342,11 +445,20 @@ class Qwen3TTSSpeechTokenizer:
         return self.encoder_model is not None
 
     def load_weights(self, weights):
+        """Decoder weights (``decoder.*``, after ``sanitize``) and, when the config has an ``encoder_config`` and the dict holds
+        ``encoder_model.*`` weights (after ``Qwen3TTSSpeechTokenizerEncoder.sanitize``), the encoder."""
+        weights = dict(weights)
         self.decoder.load_weights(weights, prefix="decoder.")
+        if self.config.encoder_config is not None and any(k.startswith("encoder_model.") for k in weights):
+            self.encoder_model = Qwen3TTSSpeechTokenizerEncoder(self.config.encoder_config, self.encoder_valid_num_quantizers,
+                                                                self.device).load_weights(weights)
         return self
 
     def encode(self, audio):
-        raise ValueError("Encoder not available for this speech tokenizer")      # same error as speech_tokenizer.py:1092-1093
+        """audio [B, 1, samples] at 24 kHz -> codes [B, 16, ceil(samples / 1920)] (speech_tokenizer.py:1082-1093)."""
+        if self.encoder_model is None:
+            raise ValueError("Encoder not available for this speech tokenizer")      # same error as speech_tokenizer.py:1092-1093
+        return self.encoder_model.encode(audio)
 
     def decode(self, audio_codes: torch.Tensor):
         """audio_codes [B, T, 16] -> (wav [B, samples], audio_lengths [B])."""
@@ -391,7 +503,7 @@ class Qwen3TTSSpeechTokenizer:
         out, codebook = {}, {}
         for k, v in weights.items():
             if k.startswith("encoder."):
-                continue                                                # encode side: SURVEY.md section 8f "next"
+                continue                                                # encode side: Qwen3TTSSpeechTokenizerEncoder.sanitize
             if "_codebook.cluster_usage" in k or "_codebook.embedding_sum" in k:
                 base = k.rsplit("._codebook.", 1)[0]
                 codebook.setdefault(base, {})["cluster_usage" if "cluster_usage" in k else "embedding_sum"] = v

@@ -20,6 +20,7 @@ from .... import ops
 from .config import Qwen3TTSTalkerCodePredictorConfig, Qwen3TTSTalkerConfig
 
 GEMV_MAX_ROWS = 16
+PREFILL_TC_MIN_ROWS = 64          # prefills of at least this many rows run attention on b2a_attn_prefill (one full query tile)
 FUSED_DECODE = [os.environ.get("B2A_LM_FUSED", "0") != "0"]       # S = 1: qk-norm + rope + cache append + attention in one launch
 # (8 CTAs walking the cache lose to 384 warps + 16 CTAs at small batch; kept for B >= 8)
 PREFETCH = [os.environ.get("B2A_LM_PREFETCH", "1") != "0"]      # pull the next projection's weights into L2 from the current GEMV
@@ -79,6 +80,9 @@ class _DecoderStack:
         x2 = x.reshape(B * S, H)
         hq, hk, hd = self.n_heads, self.n_kv, self.hd
         max_k = self.kc.shape[2] if base_dev is not None else base + S
+        # long prefills (the in-context cloning prompt) on the tensor-core kernel; decode frames, the code predictor and short prompts
+        # stay on attn_decode
+        prefill_tc = S >= PREFILL_TC_MIN_ROWS and hd == 128 and hq == 2 * hk
         for li, lw in enumerate(self.layers):
             nxt_qkv = self.layers[li + 1]["qkv"] if li + 1 < len(self.layers) else tail
             qkv = self._proj(x2, lw["qkv"], norm_w=lw["n1"], nxt=lw["o"])
@@ -90,8 +94,9 @@ class _DecoderStack:
                 q = ops.qknorm_rope_cache(qkv.view(B, S, -1), hq, hk, hd, self.kc[li], self.vc[li], q_norm=lw["qn"], k_norm=lw["kn"],
                                           eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
                                           pos_shift=pos_shift)
-                a = ops.attn_decode(q, self.kc[li], self.vc[li], hq, hk, hd, scale=hd ** -0.5, base_dev=base_dev, base=base,
-                                    kv_start=kv_start, max_k=max_k)
+                attn = ops.attn_prefill if prefill_tc else ops.attn_decode
+                a = attn(q, self.kc[li], self.vc[li], hq, hk, hd, scale=hd ** -0.5, base_dev=base_dev, base=base, kv_start=kv_start,
+                         max_k=max_k)
             x2 = self._proj(a.view(B * S, hq * hd), lw["o"], res=x2, nxt=lw["gu"])
             m = self._proj(x2, lw["gu"], norm_w=lw["n2"], swiglu=True, nxt=lw["down"])
             x2 = self._proj(m, lw["down"], res=x2, nxt=nxt_qkv)
