@@ -313,34 +313,44 @@ int32_t b2a_gemv_bf16(const float* x, int64_t x_ld, int32_t M, int32_t K, const 
  * base = *base_dev (or base_host when base_dev is NULL).  Rotary position of frequency slot i: pos3[axis,b,s] with the
  * interleaved-MRoPE axis rule of talker.py:139-184 (axis 1 if i%3==1 && i<3*sec_h, axis 2 if i%3==2 && i<3*sec_w, else 0);
  * pos3 NULL = base + s on every axis (sec_h = sec_w = 0 gives the standard RoPE of talker.py:68-113), minus pos_shift[b] (clamped at
- * 0) when pos_shift != NULL: the cumsum(attention_mask) - 1 positions of left-padded batches (talker.py:452-457). */
+ * 0) when pos_shift != NULL: the cumsum(attention_mask) - 1 positions of left-padded batches (talker.py:452-457).
+ * Per-row cache positions (continuous batching, replacing the KVCache.merge / BatchKVCache.extract of continuous_batching.py:140,178,
+ * 309-324, and the attention_mask of :280-302): base_rows [B] != NULL takes the place of the scalar base, so row b, query s goes to cache
+ * row and rotary position base_rows[b] + s; a negative value is a left-padding row and writes nothing.  slot [B] != NULL is the cache
+ * batch index row b reads and writes (NULL = b).  Both NULL: unchanged behaviour. */
 int32_t b2a_qknorm_rope_cache(const float* qkv, int64_t qkv_bs, int64_t qkv_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
                               int32_t D, const float* q_norm_w, const float* k_norm_w, float eps, const int32_t* pos3,
                               const int32_t* base_dev, int32_t base_host, int32_t sec_h, int32_t sec_w, float theta,
                               float* q_out, int64_t qo_bs, int64_t qo_ss, float* k_cache, float* v_cache, int64_t c_bs,
-                              int64_t c_ss, int32_t smax, const int32_t* pos_shift, void* stream);
+                              int64_t c_ss, int32_t smax, const int32_t* pos_shift, const int32_t* base_rows, const int32_t* slot,
+                              void* stream);
 /* mx.fast.scaled_dot_product_attention against the KV cache with GQA (talker.py:309-312): query s attends cache rows
  * [kv_start[b], base + s] (causal inside the new block; kv_start NULL = 0, else the left-padding count of
- * qwen3_tts.py:486-604's batches).  out [B,S,Hq*D].  max_k bounds base + S (shared-memory sizing). */
+ * qwen3_tts.py:486-604's batches).  out [B,S,Hq*D].  max_k bounds base + S (shared-memory sizing).  base_rows / slot as in
+ * b2a_qknorm_rope_cache: query s of row b sees cache rows [kv_start[b], base_rows[b] + s] of cache batch slot[b]; a query whose
+ * position is negative (left padding) has a zero output. */
 int32_t b2a_attn_decode(const float* q, int64_t q_bs, int64_t q_ss, const float* k_cache, const float* v_cache, int64_t c_bs,
                         int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
                         int32_t D, float scale, const int32_t* base_dev, int32_t base_host, const int32_t* kv_start,
-                        int32_t max_k, void* stream);
+                        int32_t max_k, const int32_t* base_rows, const int32_t* slot, void* stream);
 /* The same contract as b2a_attn_decode for long prefills (talker.py:288-312 over a prompt of >= 64 rows: the in-context voice-cloning
  * prompt) on the tensor cores: head_dim 128, Hq = 2 Hkv.  One CTA per (64 query rows, kv head, batch row); both query heads of the GQA
  * pair share each K / V tile, which is read once from the fp32 cache and split into fp16 hi / lo planes (3-product scores and P V,
  * fp32 accumulate).  Keys are taken in a fixed order: bit-reproducible.  Query row s sees cache rows [kv_start[b], min(base + s,
- * max_k - 1)].  Rows 16-byte aligned (q, caches); out rows 8-byte aligned. */
+ * max_k - 1)].  Rows 16-byte aligned (q, caches); out rows 8-byte aligned.  base_rows / slot as in b2a_attn_decode; key tiles
+ * outside a CTA's ragged key range (including tiles whose query rows are all left padding) are skipped, not masked. */
 int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, const float* k_cache, const float* v_cache, int64_t c_bs,
                          int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
                          int32_t D, float scale, const int32_t* base_dev, int32_t base_host, const int32_t* kv_start,
-                         int32_t max_k, void* stream);
+                         int32_t max_k, const int32_t* base_rows, const int32_t* slot, void* stream);
 /* Single-token decode (S = 1, GQA group of 2): b2a_qknorm_rope_cache + b2a_attn_decode in one launch, one CTA per (kv head, batch)
- * -- each cache row is read once for both query heads of the group.  qkv [B, (Hq+2Hkv) D]; out [B, Hq*D]; pos3 [3,B] or NULL. */
+ * -- each cache row is read once for both query heads of the group.  qkv [B, (Hq+2Hkv) D]; out [B, Hq*D]; pos3 [3,B] or NULL.
+ * base_rows / slot as in b2a_qknorm_rope_cache (a negative base writes nothing and gives a zero output). */
 int32_t b2a_attn_decode_fused(const float* qkv, int64_t qkv_bs, int32_t B, int32_t Hq, int32_t Hkv, int32_t D, const float* q_norm_w,
                               const float* k_norm_w, float eps, const int32_t* pos3, const int32_t* base_dev, int32_t base_host,
                               int32_t sec_h, int32_t sec_w, float theta, float* k_cache, float* v_cache, int64_t c_bs, int64_t c_ss,
-                              int32_t smax, float scale, const int32_t* kv_start, float* out, int64_t o_bs, void* stream);
+                              int32_t smax, float scale, const int32_t* kv_start, float* out, int64_t o_bs, const int32_t* base_rows,
+                              const int32_t* slot, void* stream);
 /* y[r, i] = silu(gate) * up (talker.py:319-321, speech_tokenizer.py:321-322) for the batched (prefill) path: x [rows, 2I] holds
  * (gate | up) halves, or interleaved (gate_0, up_0, gate_1, ...) pairs -- the row order b2a_gemv_bf16 mode 1 uses. */
 int32_t b2a_swiglu(const float* x, int64_t x_ld, int64_t rows, int32_t I, int32_t interleaved, float* y, int64_t y_ld, void* stream);
@@ -355,6 +365,13 @@ int32_t b2a_embed_sum(const int64_t* codes, int64_t codes_bs, int32_t B, int32_t
                       int32_t* err_flag_dev, int32_t* tidx, const uint8_t* finished, void* stream);
 /* *p += v on the stream (KVCache.offset bookkeeping, lm/models/cache.py:112-155, kept on the device). */
 int32_t b2a_incr_i32(int32_t* p, int32_t v, void* stream);
+/* End of a continuous-batching frame over B slots (the per-request bookkeeping of _advance_active, continuous_batching.py:201-216):
+ * for every slot whose finished[b] is 0 after the frame's sample (the sampler sets it on EOS; empty slots are kept at 1),
+ * out[b, frames[b], :] = codes[b, :G] (out row stride out_bs), frames[b] += 1, lengths[b] += 1, finished[b] = 1 once
+ * frames[b] >= cap[b] (the max_tokens test of :210-213), else u[g, b] = u_tab[b, frames[b], g] (row stride u_bs) for the next
+ * frame.  Finished and empty slots are unchanged, so a CUDA graph of the frame needs no host scalar. */
+int32_t b2a_slot_advance(int32_t* lengths, int32_t* frames, uint8_t* finished, const int32_t* cap, const int64_t* codes, int32_t G,
+                         int64_t* out, int64_t out_bs, const float* u_tab, int64_t u_bs, float* u, int32_t B, void* stream);
 
 /* ---- codec (RVQ decode) ---------------------------------------------------------------------
  * out[b,t,:] (+)= sum_q codebooks[q][codes[b,q,t]][:]   (mimi/modules/quantization.py:47-49,103-108;

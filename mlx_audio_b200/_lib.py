@@ -111,14 +111,17 @@ PROTOTYPES = {
     "b2a_sample_token": (i32, [c_f, i64, i32, i32, c_f, c_f, i64, i32, f32, f32, i32, f32, f32, c_f, c_f, i64, c_f, c_f, i32, C.c_void_p]),
     "b2a_gemv_bf16": (i32, [c_f, i64, i32, i32, c_f, i64, i32, c_f, c_f, f32, i32, c_f, i64, c_f, i64, c_f, i64, C.c_void_p]),
     "b2a_qknorm_rope_cache": (i32, [c_f, i64, i64, i32, i32, i32, i32, i32, c_f, c_f, f32, c_f, c_f, i32, i32, i32, f32, c_f, i64, i64,
-                                    c_f, c_f, i64, i64, i32, c_f, C.c_void_p]),
-    "b2a_attn_decode": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, C.c_void_p]),
-    "b2a_attn_prefill": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, C.c_void_p]),
+                                    c_f, c_f, i64, i64, i32, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_attn_decode": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, c_f, c_f,
+                              C.c_void_p]),
+    "b2a_attn_prefill": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, c_f, c_f,
+                               C.c_void_p]),
     "b2a_attn_decode_fused": (i32, [c_f, i64, i32, i32, i32, i32, c_f, c_f, f32, c_f, c_f, i32, i32, i32, f32, c_f, c_f, i64, i64, i32, f32,
-                                    c_f, c_f, i64, C.c_void_p]),
+                                    c_f, c_f, i64, c_f, c_f, C.c_void_p]),
     "b2a_swiglu": (i32, [c_f, i64, i64, i32, i32, c_f, i64, C.c_void_p]),
     "b2a_embed_sum": (i32, [c_f, i64, i32, i32, i32, c_f, c_f, c_f, i64, i64, i32, c_f, c_f, i32, c_f, i64, c_f, c_f, c_f, C.c_void_p]),
     "b2a_incr_i32": (i32, [c_f, i32, C.c_void_p]),
+    "b2a_slot_advance": (i32, [c_f, c_f, c_f, c_f, c_f, i32, c_f, i64, c_f, i64, c_f, i32, C.c_void_p]),
     "b2a_rvq_decode": (i32, [c_f, i64, i64, i32, i32, i64, c_f, i32, i32, c_f, i64, c_f, C.c_void_p]),
     "b2a_rvq_encode": (i32, [c_f, i64, i64, i32, c_f, c_f, i32, i32, i32, c_f, i64, i64, C.c_void_p]),
     "b2a_snac_from_codes": (i32, [C.POINTER(C.c_void_p), C.POINTER(i32), i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),

@@ -31,6 +31,7 @@ struct PfParams {
   float* o; int64_t o_bs, o_ss;                    // [B, S, Hq*128]
   int S, Hkv; float qmul;                          // qmul = scale * log2(e)
   const int* base_dev; int base_host; const int* kv_start; int max_k;
+  const int* base_rows; const int* slot;           // [B] per-row base (negative query positions: zero output) and cache batch index
 };
 
 // D[64 x 128] (+)= A[64 x 16] (fp16, registers) * B[16 x 128] (fp16, shared memory, K-major)
@@ -71,10 +72,10 @@ __device__ __forceinline__ void split8(const float* src, float mul, uint4& hi, u
 // K / V rows [kt, kt + 64) of KV head hk into one stage; rows outside [klo, khi) are zero (never read from the cache).
 // Thread t owns key kt + (t & 63) and dim groups (t >> 6) + 4 i: a warp covers 32 keys of one dim group, so the transposed V stores of
 // a warp hit 16 distinct words and the K stores fill whole 128-byte wavefronts.
-__device__ __forceinline__ void load_kv(uint8_t* st, const PfParams& p, int b, int hk, int kt, int klo, int khi) {
+__device__ __forceinline__ void load_kv(uint8_t* st, const PfParams& p, int cb, int hk, int kt, int klo, int khi) {
   const int j = threadIdx.x & 63, key = kt + j;
   const bool ok = key >= klo && key < khi;
-  const int64_t row = (int64_t)b * p.c_bs + (int64_t)key * p.c_ss + (int64_t)hk * HD;
+  const int64_t row = (int64_t)cb * p.c_bs + (int64_t)key * p.c_ss + (int64_t)hk * HD;
 #pragma unroll 2
   for (int i = 0; i < 4; i++) {
     const int c8 = (threadIdx.x >> 6) + 4 * i;                    // dims [8 c8, 8 c8 + 8)
@@ -104,10 +105,12 @@ __global__ void __launch_bounds__(THREADS, 1) attn_prefill_kernel(const PfParams
   const int wg = warp >> 2, w4 = warp & 3;
   const int q0 = blockIdx.x * BM, hk = blockIdx.y, b = blockIdx.z;
   pdl_wait();                                                    // q and the cache rows are the predecessor's output
-  const int base = p.base_dev ? *p.base_dev : p.base_host;
+  const int base = p.base_rows ? p.base_rows[b] : (p.base_dev ? *p.base_dev : p.base_host);
+  const int cb = p.slot ? p.slot[b] : b;
   const int klo = p.kv_start ? p.kv_start[b] : 0;
   const int rows = p.S - q0 < BM ? p.S - q0 : BM;
-  int khi = base + q0 + rows;                                    // keys [klo, khi) can be seen by some row of this tile
+  int khi = base + q0 + rows;                                    // keys [klo, khi) can be seen by some row of this tile (none when
+                                                                 // every row is left padding: base + q0 + rows <= 0)
   if (khi > p.max_k) khi = p.max_k;
   const int t_lo = klo / BN, t_hi = (khi + BN - 1) / BN;
   const int nt = khi > klo ? t_hi - t_lo : 0;
@@ -121,7 +124,7 @@ __global__ void __launch_bounds__(THREADS, 1) attn_prefill_kernel(const PfParams
     *reinterpret_cast<uint4*>(t) = hi;
     *reinterpret_cast<uint4*>(t + 2 * Q_TILE) = lo;
   }
-  if (nt > 0) load_kv(smem + OFF_KV, p, b, hk, t_lo * BN, klo, khi);
+  if (nt > 0) load_kv(smem + OFF_KV, p, cb, hk, t_lo * BN, klo, khi);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the wgmma operand reads
   __syncthreads();
 
@@ -151,7 +154,7 @@ __global__ void __launch_bounds__(THREADS, 1) attn_prefill_kernel(const PfParams
       wgmma_chunk<2, true>(sc, dqh, dkl, 1u);
     }
     wgmma_commit();
-    if (t + 1 < nt) load_kv(smem + OFF_KV + (s ^ 1) * KV_STAGE, p, b, hk, kt + BN, klo, khi);   // overlaps the score MMAs
+    if (t + 1 < nt) load_kv(smem + OFF_KV + (s ^ 1) * KV_STAGE, p, cb, hk, kt + BN, klo, khi);   // overlaps the score MMAs
     wgmma_wait<0>();
     wgmma_fence_regs<32>(sc);
     // mask + row max (element 4j + e: row h = e >> 1, key kt + 8j + 2 (lane % 4) + (e & 1))
@@ -238,7 +241,8 @@ __global__ void __launch_bounds__(THREADS, 1) attn_prefill_kernel(const PfParams
 extern "C" int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, const float* k_cache, const float* v_cache,
                                     int64_t c_bs, int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S,
                                     int32_t Hq, int32_t Hkv, int32_t D, float scale, const int32_t* base_dev, int32_t base_host,
-                                    const int32_t* kv_start, int32_t max_k, void* stream) {
+                                    const int32_t* kv_start, int32_t max_k, const int32_t* base_rows, const int32_t* slot,
+                                    void* stream) {
   B2A_CHECK_ARG(q && k_cache && v_cache && out, "null pointer");
   B2A_CHECK_ARG(D == HD && Hq == 2 * Hkv, "tensor-core prefill attention: head_dim 128, two query heads per KV head");
   B2A_CHECK_ARG(B > 0 && S > 0 && Hkv > 0 && max_k > 0 && c_ss >= (int64_t)Hkv * D, "bad shape");
@@ -247,7 +251,7 @@ extern "C" int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, 
                 "cache rows must be 16-byte aligned");
   B2A_CHECK_ARG(o_ss % 2 == 0 && o_bs % 2 == 0 && ((uintptr_t)out & 7) == 0, "out rows must be 8-byte aligned");
   PfParams p{q, q_bs, q_ss, k_cache, v_cache, c_bs, c_ss, out, o_bs, o_ss, S, Hkv, scale * 1.4426950408889634f,
-             base_dev, base_host, kv_start, max_k};
+             base_dev, base_host, kv_start, max_k, base_rows, slot};
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(attn_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); attr = true; }
   dim3 grid((unsigned)((S + BM - 1) / BM), (unsigned)Hkv, (unsigned)B);

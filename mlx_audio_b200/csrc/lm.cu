@@ -277,6 +277,7 @@ struct QkParams {
   const int* pos3; const int* base_dev; int base_host;
   int sec_h, sec_w; float theta;
   const int* pos_shift;                            // [B] left-padding count: rotary position = max(cache row - pos_shift[b], 0) (qwen3 batches)
+  const int* base_rows; const int* slot;           // [B] per-row base (negative row = left padding: no write) and cache batch index
   float* q_out; int64_t qo_bs, qo_ss;              // [B,S,Hq,D]
   float* kc; float* vc; int64_t c_bs, c_ss;        // caches [B,Smax,Hkv,D]
   int smax;
@@ -293,15 +294,16 @@ __global__ void qknorm_rope_cache_kernel(const QkParams p) {
   if (wid >= (int64_t)p.B * p.S * HT) return;
   const int h = (int)(wid % HT);
   const int s = (int)((wid / HT) % p.S), b = (int)(wid / ((int64_t)HT * p.S));
-  const int base = p.base_dev ? *p.base_dev : p.base_host;
+  const int base = p.base_rows ? p.base_rows[b] : (p.base_dev ? *p.base_dev : p.base_host);
   const int cpos = base + s;
+  const int cb = p.slot ? p.slot[b] : b;
   const float* src = p.qkv + (int64_t)b * p.qkv_bs + (int64_t)s * p.qkv_ss + (int64_t)h * D;
   float v[E];
 #pragma unroll
   for (int j = 0; j < E; j++) v[j] = src[lane + 32 * j];
   if (h >= p.Hq + p.Hkv) {                         // v head: straight into the cache
-    if (cpos < p.smax) {
-      float* dst = p.vc + (int64_t)b * p.c_bs + (int64_t)cpos * p.c_ss + (int64_t)(h - p.Hq - p.Hkv) * D;
+    if (cpos >= 0 && cpos < p.smax) {
+      float* dst = p.vc + (int64_t)cb * p.c_bs + (int64_t)cpos * p.c_ss + (int64_t)(h - p.Hq - p.Hkv) * D;
 #pragma unroll
       for (int j = 0; j < E; j++) dst[lane + 32 * j] = v[j];
     }
@@ -349,8 +351,8 @@ __global__ void qknorm_rope_cache_kernel(const QkParams p) {
     float* dst = p.q_out + (int64_t)b * p.qo_bs + (int64_t)s * p.qo_ss + (int64_t)h * D;
 #pragma unroll
     for (int j = 0; j < E; j++) dst[lane + 32 * j] = o[j];
-  } else if (cpos < p.smax) {
-    float* dst = p.kc + (int64_t)b * p.c_bs + (int64_t)cpos * p.c_ss + (int64_t)(h - p.Hq) * D;
+  } else if (cpos >= 0 && cpos < p.smax) {
+    float* dst = p.kc + (int64_t)cb * p.c_bs + (int64_t)cpos * p.c_ss + (int64_t)(h - p.Hq) * D;
 #pragma unroll
     for (int j = 0; j < E; j++) dst[lane + 32 * j] = o[j];
   }
@@ -366,6 +368,7 @@ struct AdParams {
   float* o; int64_t o_bs, o_ss;
   int B, S, Hq, Hkv; float scale;
   const int* base_dev; int base_host; const int* kv_start; int max_k;
+  const int* base_rows; const int* slot;           // [B] per-row base (base + s < 0: zero output) and cache batch index
 };
 
 constexpr int AD_THREADS = 256;
@@ -379,7 +382,8 @@ __global__ void __launch_bounds__(AD_THREADS) attn_decode_kernel(const AdParams 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   pdl_launch_dependents();
   pdl_wait();
-  const int base = p.base_dev ? *p.base_dev : p.base_host;
+  const int base = p.base_rows ? p.base_rows[b] : (p.base_dev ? *p.base_dev : p.base_host);
+  const int cb = p.slot ? p.slot[b] : b;
   int klen = base + s + 1;
   if (klen > p.max_k) klen = p.max_k;
   const int k0 = p.kv_start ? p.kv_start[b] : 0;
@@ -388,8 +392,8 @@ __global__ void __launch_bounds__(AD_THREADS) attn_decode_kernel(const AdParams 
   float qv[E];
 #pragma unroll
   for (int j = 0; j < E; j++) qv[j] = qp[lane * E + j] * p.scale;
-  const float* kb = p.kc + (int64_t)b * p.c_bs + (int64_t)hk * D;
-  const float* vb = p.vc + (int64_t)b * p.c_bs + (int64_t)hk * D;
+  const float* kb = p.kc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
+  const float* vb = p.vc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
   float mloc = -INFINITY;
   for (int j = k0 + warp; j < klen; j += NW) {
     const float* kr = kb + (int64_t)j * p.c_ss + lane * E;
@@ -449,6 +453,7 @@ struct FdParams {
   const int* pos3; const int* base_dev; int base_host; int sec_h, sec_w; float theta;
   float* kc; float* vc; int64_t c_bs, c_ss; int smax;
   float* o; int64_t o_bs; float scale; const int* kv_start;
+  const int* base_rows; const int* slot;           // [B] per-row base (negative: no write, zero output) and cache batch index
 };
 
 template <int D, int G>
@@ -461,12 +466,13 @@ __global__ void __launch_bounds__(256) attn_decode_fused_kernel(const FdParams p
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   pdl_launch_dependents();
   pdl_wait();
-  const int base = p.base_dev ? *p.base_dev : p.base_host;
+  const int base = p.base_rows ? p.base_rows[b] : (p.base_dev ? *p.base_dev : p.base_host);
   const int klen = min(base + 1, p.smax);
   const int k0 = p.kv_start ? p.kv_start[b] : 0;
+  const int cb = p.slot ? p.slot[b] : b;
   const float* row = p.qkv + (int64_t)b * p.qkv_bs;
-  float* kb = p.kc + (int64_t)b * p.c_bs + (int64_t)hk * D;
-  float* vb = p.vc + (int64_t)b * p.c_bs + (int64_t)hk * D;
+  float* kb = p.kc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
+  float* vb = p.vc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
   // ---- phase A: prepare q (G heads), k, v
   if (warp < G + 2) {
     const bool is_v = warp == 1, is_k = warp == 0;
@@ -476,7 +482,7 @@ __global__ void __launch_bounds__(256) attn_decode_fused_kernel(const FdParams p
 #pragma unroll
     for (int j = 0; j < E; j++) v[j] = src[lane + 32 * j];
     if (is_v) {
-      if (base < p.smax) {
+      if (base >= 0 && base < p.smax) {
 #pragma unroll
         for (int j = 0; j < E; j++) vb[(int64_t)base * p.c_ss + lane + 32 * j] = v[j];
       }
@@ -506,7 +512,7 @@ __global__ void __launch_bounds__(256) attn_decode_fused_kernel(const FdParams p
         o[j + E / 2] = v[j + E / 2] * c + v[j] * sf;
       }
       if (is_k) {
-        if (base < p.smax) {
+        if (base >= 0 && base < p.smax) {
 #pragma unroll
           for (int j = 0; j < E; j++) kb[(int64_t)base * p.c_ss + lane + 32 * j] = o[j];
         }
@@ -652,6 +658,23 @@ __global__ void advance_tidx_kernel(int* tidx, const uint8_t* finished, int B) {
 
 __global__ void incr_kernel(int* p, int v) { pdl_launch_dependents(); pdl_wait(); *p += v; }
 
+// End of a batch-session frame, one thread per slot.  A slot that is not finished after this frame's sample (EOS sets the flag in
+// the sampler; empty slots are kept finished) records its codes at its frame count, advances its cache length and frame count,
+// finishes at its frame cap, and loads its next frame's uniforms.  Finished and empty slots are left unchanged.
+__global__ void slot_advance_kernel(int* lengths, int* frames, uint8_t* finished, const int* cap, const int64_t* codes, int G,
+                                    int64_t* out, int64_t out_bs, const float* u_tab, int64_t u_bs, float* u, int B) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || finished[b]) return;
+  const int f = frames[b];
+  for (int g = 0; g < G; g++) out[(int64_t)b * out_bs + (int64_t)f * G + g] = codes[(int64_t)b * G + g];
+  frames[b] = f + 1;
+  lengths[b] += 1;
+  if (f + 1 >= cap[b]) { finished[b] = 1; return; }
+  for (int g = 0; g < G; g++) u[(int64_t)g * B + b] = u_tab[(int64_t)b * u_bs + (int64_t)(f + 1) * G + g];
+}
+
 }  // namespace
 
 extern "C" int32_t b2a_gemv_bf16(const float* x, int64_t x_ld, int32_t M, int32_t K, const void* w_bf16, int64_t w_ld, int32_t N,
@@ -683,11 +706,12 @@ extern "C" int32_t b2a_qknorm_rope_cache(const float* qkv, int64_t qkv_bs, int64
                                          int32_t Hkv, int32_t D, const float* q_norm_w, const float* k_norm_w, float eps,
                                          const int32_t* pos3, const int32_t* base_dev, int32_t base_host, int32_t sec_h,
                                          int32_t sec_w, float theta, float* q_out, int64_t qo_bs, int64_t qo_ss, float* k_cache,
-                                         float* v_cache, int64_t c_bs, int64_t c_ss, int32_t smax, const int32_t* pos_shift, void* stream) {
+                                         float* v_cache, int64_t c_bs, int64_t c_ss, int32_t smax, const int32_t* pos_shift,
+                                         const int32_t* base_rows, const int32_t* slot, void* stream) {
   B2A_CHECK_ARG(D == 32 || D == 64 || D == 128, "head_dim must be 32, 64 or 128");
   B2A_CHECK_ARG(B > 0 && S > 0 && Hq > 0 && Hkv > 0 && Hq % Hkv == 0, "bad shape");
   QkParams p{qkv, qkv_bs, qkv_ss, B, S, Hq, Hkv, D, q_norm_w, k_norm_w, eps, pos3, base_dev, base_host, sec_h, sec_w, theta, pos_shift,
-             q_out, qo_bs, qo_ss, k_cache, v_cache, c_bs, c_ss, smax};
+             base_rows, slot, q_out, qo_bs, qo_ss, k_cache, v_cache, c_bs, c_ss, smax};
   const int64_t warps = (int64_t)B * S * (Hq + 2 * Hkv);
   const int grid = (int)((warps * 32 + 255) / 256);
   if (D == 128) b2a_launch_pdl(qknorm_rope_cache_kernel<128>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, p);
@@ -700,11 +724,12 @@ extern "C" int32_t b2a_qknorm_rope_cache(const float* qkv, int64_t qkv_bs, int64
 extern "C" int32_t b2a_attn_decode(const float* q, int64_t q_bs, int64_t q_ss, const float* k_cache, const float* v_cache,
                                    int64_t c_bs, int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S,
                                    int32_t Hq, int32_t Hkv, int32_t D, float scale, const int32_t* base_dev, int32_t base_host,
-                                   const int32_t* kv_start, int32_t max_k, void* stream) {
+                                   const int32_t* kv_start, int32_t max_k, const int32_t* base_rows, const int32_t* slot, void* stream) {
   B2A_CHECK_ARG(D == 32 || D == 64 || D == 128, "head_dim must be 32, 64 or 128");
   B2A_CHECK_ARG(B > 0 && S > 0 && Hq % Hkv == 0 && max_k > 0 && max_k <= 48 * 1024, "bad shape (max_k <= 49152)");
   B2A_CHECK_ARG(c_ss % 4 == 0 && c_bs % 4 == 0 && ((uintptr_t)k_cache & 15) == 0 && ((uintptr_t)v_cache & 15) == 0, "cache rows must be 16-byte aligned");
-  AdParams p{q, q_bs, q_ss, k_cache, v_cache, c_bs, c_ss, out, o_bs, o_ss, B, S, Hq, Hkv, scale, base_dev, base_host, kv_start, max_k};
+  AdParams p{q, q_bs, q_ss, k_cache, v_cache, c_bs, c_ss, out, o_bs, o_ss, B, S, Hq, Hkv, scale, base_dev, base_host, kv_start, max_k,
+              base_rows, slot};
   size_t floats = (size_t)max_k;
   if (floats < (size_t)(AD_THREADS / 32) * D) floats = (size_t)(AD_THREADS / 32) * D;
   const size_t sm = floats * sizeof(float);
@@ -728,12 +753,13 @@ extern "C" int32_t b2a_attn_decode_fused(const float* qkv, int64_t qkv_bs, int32
                                          const float* q_norm_w, const float* k_norm_w, float eps, const int32_t* pos3,
                                          const int32_t* base_dev, int32_t base_host, int32_t sec_h, int32_t sec_w, float theta,
                                          float* k_cache, float* v_cache, int64_t c_bs, int64_t c_ss, int32_t smax, float scale,
-                                         const int32_t* kv_start, float* out, int64_t o_bs, void* stream) {
+                                         const int32_t* kv_start, float* out, int64_t o_bs, const int32_t* base_rows,
+                                         const int32_t* slot, void* stream) {
   B2A_CHECK_ARG((D == 64 || D == 128) && Hq == 2 * Hkv, "fused decode attention: head_dim 64/128 and a 2:1 GQA group");
   B2A_CHECK_ARG(B > 0 && smax > 0 && smax <= 24 * 1024, "bad shape (cache rows <= 24576)");
   B2A_CHECK_ARG(c_ss % 4 == 0 && c_bs % 4 == 0 && ((uintptr_t)k_cache & 15) == 0 && ((uintptr_t)v_cache & 15) == 0, "cache rows must be 16-byte aligned");
   FdParams p{qkv, qkv_bs, B, Hq, Hkv, q_norm_w, k_norm_w, eps, pos3, base_dev, base_host, sec_h, sec_w, theta, k_cache, v_cache, c_bs, c_ss,
-             smax, out, o_bs, scale, kv_start};
+             smax, out, o_bs, scale, kv_start, base_rows, slot};
   size_t floats = (size_t)2 * smax;
   if (floats < (size_t)8 * 2 * D) floats = (size_t)8 * 2 * D;
   const size_t sm = floats * sizeof(float);
@@ -770,6 +796,17 @@ extern "C" int32_t b2a_embed_sum(const int64_t* codes, int64_t codes_bs, int32_t
   dim3 grid((dim + 255) / 256, B);
   b2a_launch_pdl(embed_sum_kernel, grid, dim3(256), 0, (cudaStream_t)stream, p);
   if (tidx) b2a_launch_pdl(advance_tidx_kernel, dim3((B + 63) / 64), dim3(64), 0, (cudaStream_t)stream, tidx, finished, (int)B);
+  B2A_CHECK_LAUNCH();
+  return B2A_OK;
+}
+
+extern "C" int32_t b2a_slot_advance(int32_t* lengths, int32_t* frames, uint8_t* finished, const int32_t* cap, const int64_t* codes,
+                                    int32_t G, int64_t* out, int64_t out_bs, const float* u_tab, int64_t u_bs, float* u, int32_t B,
+                                    void* stream) {
+  B2A_CHECK_ARG(lengths && frames && finished && cap && codes && out && u_tab && u, "null pointer");
+  B2A_CHECK_ARG(B > 0 && G > 0 && out_bs >= G && u_bs >= G, "bad shape");
+  b2a_launch_pdl(slot_advance_kernel, dim3((B + 63) / 64), dim3(64), 0, (cudaStream_t)stream, (int*)lengths, (int*)frames, finished,
+                 (const int*)cap, codes, (int)G, out, out_bs, u_tab, u_bs, u, (int)B);
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }

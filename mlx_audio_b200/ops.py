@@ -946,8 +946,10 @@ def gemv(x: torch.Tensor, cw: "ConvW", *, norm_w=None, norm_eps: float = 1e-6, s
 
 def qknorm_rope_cache(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, k_cache: torch.Tensor, v_cache: torch.Tensor, *,
                       q_norm=None, k_norm=None, eps: float = 1e-6, pos3=None, base_dev=None, base: int = 0, mrope=(0, 0),
-                      theta: float = 10000.0, q_out=None, pos_shift=None) -> torch.Tensor:
-    """qkv [B,S,(Hq+2Hkv)D] -> q_out [B,S,Hq*D] (normed + rotated), k/v appended to caches [B,Smax,Hkv*D] at row base+s."""
+                      theta: float = 10000.0, q_out=None, pos_shift=None, base_rows=None, slot=None) -> torch.Tensor:
+    """qkv [B,S,(Hq+2Hkv)D] -> q_out [B,S,Hq*D] (normed + rotated), k/v appended to caches [B,Smax,Hkv*D] at row base+s.
+    ``base_rows`` int32 [B]: per-row base (a negative row position is left padding and writes nothing); ``slot`` int32 [B]: the
+    cache batch index of each row."""
     _chk3(qkv, "qkv")
     B, S, _ = qkv.shape
     if q_out is None:
@@ -956,44 +958,47 @@ def qknorm_rope_cache(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int,
     assert pos3 is None or (pos3.dtype == torch.int32 and pos3.is_contiguous() and pos3.shape == (3, B, S))
     _call("rope", _lib.lib().b2a_qknorm_rope_cache, 1, qkv.data_ptr(), qkv.stride(0), qkv.stride(1), B, S, n_heads, n_kv, head_dim,
           _p(q_norm), _p(k_norm), eps, _p(pos3), _p(base_dev), base, mrope[0], mrope[1], theta, q_out.data_ptr(), q_out.stride(0),
-          q_out.stride(1), k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0), k_cache.stride(1), k_cache.shape[1], _p(pos_shift), _stream())
+          q_out.stride(1), k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0), k_cache.stride(1), k_cache.shape[1], _p(pos_shift),
+          _p(_rows_i32(base_rows, B)), _p(_rows_i32(slot, B)), _stream())
     return q_out
 
 
 def attn_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, *, scale: float,
-                base_dev=None, base: int = 0, kv_start=None, max_k: Optional[int] = None, out=None) -> torch.Tensor:
-    """Causal GQA attention of q [B,S,Hq*D] against cache rows [kv_start, base+s]; out [B,S,Hq*D]."""
+                base_dev=None, base: int = 0, kv_start=None, max_k: Optional[int] = None, out=None, base_rows=None, slot=None) -> torch.Tensor:
+    """Causal GQA attention of q [B,S,Hq*D] against cache rows [kv_start, base+s]; out [B,S,Hq*D].  ``base_rows`` / ``slot`` as in
+    ``qknorm_rope_cache`` (a negative query position gives a zero row)."""
     _chk3(q, "q")
     B, S, _ = q.shape
     if out is None:
         out = torch.empty(B, S, n_heads * head_dim, device=q.device, dtype=torch.float32)
     if max_k is None:
-        max_k = k_cache.shape[1] if base_dev is not None else base + S
+        max_k = k_cache.shape[1] if base_dev is not None or base_rows is not None else base + S
     _call("attention", _lib.lib().b2a_attn_decode, 1, q.data_ptr(), q.stride(0), q.stride(1), k_cache.data_ptr(), v_cache.data_ptr(),
           k_cache.stride(0), k_cache.stride(1), out.data_ptr(), out.stride(0), out.stride(1), B, S, n_heads, n_kv, head_dim, scale,
-          _p(base_dev), base, _p(kv_start), max_k, _stream())
+          _p(base_dev), base, _p(kv_start), max_k, _p(_rows_i32(base_rows, B)), _p(_rows_i32(slot, B)), _stream())
     return out
 
 
 def attn_prefill(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, *, scale: float,
-                 base_dev=None, base: int = 0, kv_start=None, max_k: Optional[int] = None, out=None) -> torch.Tensor:
+                 base_dev=None, base: int = 0, kv_start=None, max_k: Optional[int] = None, out=None, base_rows=None, slot=None) -> torch.Tensor:
     """``attn_decode``'s contract on the tensor cores, for prefills of >= 64 rows with head_dim 128 and two query heads per KV head."""
     _chk3(q, "q")
     B, S, _ = q.shape
     if out is None:
         out = torch.empty(B, S, n_heads * head_dim, device=q.device, dtype=torch.float32)
     if max_k is None:
-        max_k = k_cache.shape[1] if base_dev is not None else base + S
+        max_k = k_cache.shape[1] if base_dev is not None or base_rows is not None else base + S
     _call("attention", _lib.lib().b2a_attn_prefill, 1, q.data_ptr(), q.stride(0), q.stride(1), k_cache.data_ptr(), v_cache.data_ptr(),
           k_cache.stride(0), k_cache.stride(1), out.data_ptr(), out.stride(0), out.stride(1), B, S, n_heads, n_kv, head_dim, scale,
-          _p(base_dev), base, _p(kv_start), max_k, _stream())
+          _p(base_dev), base, _p(kv_start), max_k, _p(_rows_i32(base_rows, B)), _p(_rows_i32(slot, B)), _stream())
     return out
 
 
 def attn_decode_fused(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, k_cache: torch.Tensor, v_cache: torch.Tensor, *, scale: float,
                       q_norm=None, k_norm=None, eps: float = 1e-6, pos3=None, base_dev=None, base: int = 0, mrope=(0, 0),
-                      theta: float = 10000.0, kv_start=None, out=None) -> torch.Tensor:
-    """Single-token decode step: qkv [B,(Hq+2Hkv)D] -> attention output [B,Hq*D]; k/v appended to the caches at row ``base``."""
+                      theta: float = 10000.0, kv_start=None, out=None, base_rows=None, slot=None) -> torch.Tensor:
+    """Single-token decode step: qkv [B,(Hq+2Hkv)D] -> attention output [B,Hq*D]; k/v appended to the caches at row ``base``
+    (``base_rows`` / ``slot`` as in ``qknorm_rope_cache``)."""
     assert qkv.dim() == 2 and qkv.stride(1) == 1 and n_heads == 2 * n_kv and k_cache.stride() == v_cache.stride()
     B = qkv.shape[0]
     if out is None:
@@ -1001,7 +1006,8 @@ def attn_decode_fused(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int,
     assert pos3 is None or (pos3.dtype == torch.int32 and pos3.is_contiguous() and pos3.numel() == 3 * B)
     _call("attention", _lib.lib().b2a_attn_decode_fused, 1, qkv.data_ptr(), qkv.stride(0), B, n_heads, n_kv, head_dim, _p(q_norm), _p(k_norm),
           eps, _p(pos3), _p(base_dev), base, mrope[0], mrope[1], theta, k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0),
-          k_cache.stride(1), k_cache.shape[1], scale, _p(kv_start), out.data_ptr(), out.stride(0), _stream())
+          k_cache.stride(1), k_cache.shape[1], scale, _p(kv_start), out.data_ptr(), out.stride(0), _p(_rows_i32(base_rows, B)),
+          _p(_rows_i32(slot, B)), _stream())
     return out
 
 
@@ -1043,6 +1049,25 @@ def embed_sum(codes: torch.Tensor, tabs: EmbedTables, *, text=None, pad=None, st
     _call("other", _lib.lib().b2a_embed_sum, 1, codes.data_ptr(), codes.stride(0), B, G, tabs.dim, tabs.ptrs.data_ptr(), tabs.bins.data_ptr(),
           _p(text), tb, ts, nt, _p(pad), _p(step_dev), step_sub, out.data_ptr(), out.stride(0), _p(err), _p(tidx), _p(finished), _stream())
     return out
+
+
+def _rows_i32(t: Optional[torch.Tensor], B: int) -> Optional[torch.Tensor]:
+    """A per-row device array (``base_rows`` / ``slot``): int32 [B], contiguous."""
+    assert t is None or (t.dtype == torch.int32 and t.is_cuda and t.is_contiguous() and t.numel() == B), "per-row arrays are int32 [B] on the device"
+    return t
+
+
+def slot_advance(lengths: torch.Tensor, frames: torch.Tensor, finished: torch.Tensor, cap: torch.Tensor, codes: torch.Tensor,
+                 out: torch.Tensor, u_tab: torch.Tensor, u: torch.Tensor) -> None:
+    """End of a batch-session frame over B slots (include/b200audio.h: b2a_slot_advance): live slots record ``codes`` [B, G] into
+    ``out`` [B, F, G] at their frame count, advance their cache length and frame count, finish at ``cap`` and load the next frame's
+    uniforms ``u`` [G, B] from ``u_tab`` [B, F, G]."""
+    B, G = codes.shape
+    assert codes.dtype == torch.int64 and codes.is_contiguous() and out.dtype == torch.int64 and out.is_contiguous() and out.shape[0] == B
+    assert finished.dtype == torch.uint8 and all(t.dtype == torch.int32 and t.numel() == B for t in (lengths, frames, cap))
+    assert u_tab.is_contiguous() and u_tab.shape[0] == B and u.is_contiguous() and u.shape == (G, B)
+    _call("other", _lib.lib().b2a_slot_advance, 1, lengths.data_ptr(), frames.data_ptr(), finished.data_ptr(), cap.data_ptr(), codes.data_ptr(),
+          G, out.data_ptr(), out.stride(0), u_tab.data_ptr(), u_tab.stride(0), u.data_ptr(), B, _stream())
 
 
 def incr_(p: torch.Tensor, v: int = 1) -> None:

@@ -294,32 +294,39 @@ class Model:
         return [i for i in range(cfg.vocab_size - 1024, cfg.vocab_size) if i != eos_token_id]
 
     # ------------------------------------------------------------------ frame loop
-    def _frame(self, x_in: torch.Tensor, sp) -> None:
-        """One pass of the loop body qwen3_tts.py:1323-1398 for every batch row; results land in the state buffers."""
+    _base_rows = None       # per-row cache lengths and slot map of a batch session's frame state (continuous_batching.py); None here
+    _slot = None
+
+    def _frame(self, x_in: torch.Tensor, sp, st=None) -> None:
+        """One pass of the loop body qwen3_tts.py:1323-1398 for every batch row; results land in the state buffers of ``st`` (the
+        model's own for generate_codes, a batch session's otherwise -- its frames run at per-row cache lengths ``st._base_rows``)."""
+        st = self if st is None else st
         t, cp = self.talker, self.talker.code_predictor
-        B = x_in.shape[0]
         g = self.config.talker_config.num_code_groups
-        logits, hidden = t(x_in, use_device_offset=True, kv_start=self._kv_start)
-        ops.sample_token(logits[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=self._u[0],
-                         suppress_mask=self._suppress, seen=self._seen, repetition_penalty=sp["repetition_penalty"], mark_seen=True,
-                         out=self._codes[:, 0], finished=self._finished, eos=sp["eos"])
-        inp0 = self._cp_in0                                                                  # [B,2,H]: (hidden, embed(token 0))
+        if st._base_rows is not None:
+            logits, hidden = t(x_in, base_rows=st._base_rows, slot=st._slot)
+        else:
+            logits, hidden = t(x_in, use_device_offset=True, kv_start=st._kv_start)
+        ops.sample_token(logits[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=st._u[0],
+                         suppress_mask=st._suppress, seen=st._seen, repetition_penalty=sp["repetition_penalty"], mark_seen=True,
+                         out=st._codes[:, 0], finished=st._finished, eos=sp["eos"])
+        inp0 = st._cp_in0                                                                    # [B,2,H]: (hidden, embed(token 0))
         ops.copy2d(hidden[:, -1], inp0[:, 0])
-        ops.embed_sum(self._codes[:, 0:1], self._tab0, out=inp0[:, 1], err=self._err)
+        ops.embed_sum(st._codes[:, 0:1], self._tab0, out=inp0[:, 1], err=st._err)
         for ci in range(g - 1):
             if ci == 0:
                 lg = cp(inp0, 0, 0)
             else:
-                e = ops.embed_sum(self._codes[:, ci:ci + 1], self._tab_cp[ci - 1], out=self._cp_in, err=self._err)
+                e = ops.embed_sum(st._codes[:, ci:ci + 1], self._tab_cp[ci - 1], out=st._cp_in, err=st._err)
                 lg = cp(e[:, None], ci + 1, ci)
-            ops.sample_token(lg[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=self._u[ci + 1],
-                             out=self._codes[:, ci + 1])
-        if self._tidx is not None:      # batch rule: per-row trailing index, clamp-pad, advance unfinished rows (qwen3_tts.py:1903-1912)
-            ops.embed_sum(self._codes, self._tabs_all, text=self._trailing, pad=self._pad, out=self._x_in[:, 0], err=self._err,
-                          tidx=self._tidx, finished=self._finished)
+            ops.sample_token(lg[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=st._u[ci + 1],
+                             out=st._codes[:, ci + 1])
+        if st._tidx is not None:        # batch rule: per-row trailing index, clamp-pad, advance unfinished rows (qwen3_tts.py:1903-1912)
+            ops.embed_sum(st._codes, self._tabs_all, text=st._trailing, pad=st._pad, out=st._x_in[:, 0], err=st._err,
+                          tidx=st._tidx, finished=st._finished)
         else:
-            ops.embed_sum(self._codes, self._tabs_all, text=self._trailing, pad=self._pad, step_dev=t.offset_dev, step_sub=self._prefill_len,
-                          out=self._x_in[:, 0], err=self._err)
+            ops.embed_sum(st._codes, self._tabs_all, text=st._trailing, pad=st._pad, step_dev=t.offset_dev, step_sub=st._prefill_len,
+                          out=st._x_in[:, 0], err=st._err)
 
     def _uniform_stream(self, seed):
         """Generator the sampler's uniforms are drawn from.  ``seed=None`` continues ONE stream owned by the model, so successive
@@ -460,6 +467,34 @@ class Model:
         return out[:, :n]
 
     # ------------------------------------------------------------------ batch generation
+    def supports_tts_batch(self, *, stream: bool = False, voice: Optional[str] = None, instruct: Optional[str] = None, ref_audio=None,
+                           ref_text: Optional[str] = None, speed: Optional[float] = 1.0, pitch: Optional[float] = 1.0, **kwargs) -> bool:
+        """qwen3_tts.py:215-251: whether a request with these settings may share a batch."""
+        if stream or speed not in (None, 1.0) or pitch not in (None, 1.0):
+            return False
+        kind = getattr(self.config, "tts_model_type", "base")
+        if ref_audio is not None or ref_text is not None:
+            return (kind == "base" and ref_audio is not None and ref_text is not None and voice is None and instruct is None
+                    and self.speech_tokenizer is not None and self.speech_tokenizer.has_encoder)
+        if kind not in ("base", "custom_voice"):
+            return False
+        if kind == "base" and instruct:
+            return False
+        if kind == "custom_voice" and not voice:
+            return False
+        return True
+
+    def supports_tts_continuous_batch(self, **kwargs) -> bool:
+        """qwen3_tts.py:253-256: as ``supports_tts_batch``, but never for reference-audio requests."""
+        if kwargs.get("ref_audio") is not None or kwargs.get("ref_text") is not None:
+            return False
+        return self.supports_tts_batch(**kwargs)
+
+    def create_tts_batch_session(self, options):
+        """qwen3_tts.py:1114-1120: a step-wise continuous-batching session (``continuous_batching.Qwen3TTSBatchSession``)."""
+        from .continuous_batching import Qwen3TTSBatchSession
+        return Qwen3TTSBatchSession(self, options)
+
     @torch.no_grad()
     def prepare_batch_inputs_from_ids(self, ids_list, language_id=None, speaker_ids=None, instruct_ids=None):
         """_prepare_batch_inputs (qwen3_tts.py:486-604) after tokenisation: left-pad the prompts with zero rows, right-pad the trailing

@@ -72,14 +72,16 @@ class _DecoderStack:
         return ops.swiglu(y, interleaved=True) if swiglu else y
 
     def forward(self, x: torch.Tensor, *, base_dev=None, base: int = 0, pos3=None, kv_start=None, final_norm: bool = True,
-                tail=None, pos_shift=None) -> torch.Tensor:
+                tail=None, pos_shift=None, base_rows=None, slot=None) -> torch.Tensor:
         """x [B,S,H] -> final-normed hidden [B,S,H] (``final_norm=False``: the residual stream, for a consumer that fuses the
         norm); appends S rows to the cache at ``base`` (device scalar or host int).  ``tail``: the projection that follows the
-        stack (head), prefetched into L2 by the last layer."""
+        stack (head), prefetched into L2 by the last layer.  ``base_rows`` / ``slot`` int32 [B]: per-row cache positions and cache
+        batch indices (continuous batching; see ops.qknorm_rope_cache)."""
         B, S, H = x.shape
         x2 = x.reshape(B * S, H)
         hq, hk, hd = self.n_heads, self.n_kv, self.hd
-        max_k = self.kc.shape[2] if base_dev is not None else base + S
+        max_k = self.kc.shape[2] if base_dev is not None or base_rows is not None else base + S
+        rows = dict(base_rows=base_rows, slot=slot) if base_rows is not None or slot is not None else {}
         # long prefills (the in-context cloning prompt) on the tensor-core kernel; decode frames, the code predictor and short prompts
         # stay on attn_decode
         prefill_tc = S >= PREFILL_TC_MIN_ROWS and hd == 128 and hq == 2 * hk
@@ -89,14 +91,14 @@ class _DecoderStack:
             if S == 1 and hq == 2 * hk and hd in (64, 128) and FUSED_DECODE[0] and pos_shift is None:
                 a = ops.attn_decode_fused(qkv, hq, hk, hd, self.kc[li], self.vc[li], scale=hd ** -0.5, q_norm=lw["qn"], k_norm=lw["kn"],
                                           eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
-                                          kv_start=kv_start)
+                                          kv_start=kv_start, **rows)
             else:
                 q = ops.qknorm_rope_cache(qkv.view(B, S, -1), hq, hk, hd, self.kc[li], self.vc[li], q_norm=lw["qn"], k_norm=lw["kn"],
                                           eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
-                                          pos_shift=pos_shift)
+                                          pos_shift=pos_shift, **rows)
                 attn = ops.attn_prefill if prefill_tc else ops.attn_decode
                 a = attn(q, self.kc[li], self.vc[li], hq, hk, hd, scale=hd ** -0.5, base_dev=base_dev, base=base, kv_start=kv_start,
-                         max_k=max_k)
+                         max_k=max_k, **rows)
             x2 = self._proj(a.view(B * S, hq * hd), lw["o"], res=x2, nxt=lw["gu"])
             m = self._proj(x2, lw["gu"], norm_w=lw["n2"], swiglu=True, nxt=lw["down"])
             x2 = self._proj(m, lw["down"], res=x2, nxt=nxt_qkv)
@@ -182,11 +184,18 @@ class Qwen3TTSTalkerForConditionalGeneration:
         self.offset_dev.zero_()
         self.offset = 0
 
-    def __call__(self, inputs_embeds: torch.Tensor, position_ids=None, kv_start=None, use_device_offset: bool = False):
+    def __call__(self, inputs_embeds: torch.Tensor, position_ids=None, kv_start=None, use_device_offset: bool = False, base_rows=None,
+                 slot=None):
         """inputs_embeds [B,S,H] -> (logits [B,S,V], hidden [B,S,H]); appends to the cache (talker.py:799-818).  ``kv_start`` int32 [B]
         = left-padding count per row: the ``attention_mask`` path of talker.py:449-476 (keys before it are masked, rotary positions are
-        cumsum(mask) - 1 = cache row - kv_start, clamped at 0)."""
+        cumsum(mask) - 1 = cache row - kv_start, clamped at 0).  ``base_rows`` int32 [B] (with an optional ``slot`` map) = per-row cache
+        lengths of a continuous batch: row b appends at cache row base_rows[b] of cache batch slot[b] and sees the rows before it; a
+        negative base left-pads the row.  The caller owns those lengths: ``offset`` is not touched."""
         B, S, _ = inputs_embeds.shape
+        if base_rows is not None:
+            h = self.stack.forward(inputs_embeds, base_rows=base_rows, slot=slot, tail=self.codec_head)
+            logits = self.stack._proj(h.reshape(B * S, -1), self.codec_head, nxt=self.code_predictor.stack.layers[0]["qkv"]).view(B, S, -1)
+            return logits, h
         pos3 = None
         if position_ids is not None:
             pos3 = position_ids.to(device=self.device, dtype=torch.int32)
