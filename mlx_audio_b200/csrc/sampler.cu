@@ -266,8 +266,9 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     }
     return;
   }
-  const float inv_t = 1.f / p.temperature;
-  for (int v = tid; v < SV; v += blockDim.x) { sv[v] = v < V ? base(v) * inv_t : NEG; si[v] = v; }
+  // logits / temperature as the reference divides: a multiply by 1 / t rounds differently for many float32 inputs (about a
+  // quarter at t = 0.9) and can split two logits that tie after the division, which moves the top-k cut
+  for (int v = tid; v < SV; v += blockDim.x) { sv[v] = v < V ? base(v) / p.temperature : NEG; si[v] = v; }
   __syncthreads();
   const bool filters_p = (p.top_p > 0.f && p.top_p < 1.f) || p.min_p > 0.f;
   if (!filters_p) {
@@ -276,7 +277,12 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     __shared__ unsigned hist[256];
     __shared__ unsigned sel_prefix, sel_remaining;
     __shared__ unsigned wcnt[32];
-    auto keyof = [](float x) -> unsigned { unsigned u = __float_as_uint(x); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); };
+    // -0.0 takes the key of +0.0: the two compare equal, so they tie and the lower index wins, as on the sorted path
+    auto keyof = [](float x) -> unsigned {
+      unsigned u = __float_as_uint(x);
+      if (u == 0x80000000u) u = 0u;
+      return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    };
     const bool use_k = p.top_k > 0 && p.top_k < V;
     if (use_k) {
       if (tid == 0) { sel_prefix = 0u; sel_remaining = (unsigned)p.top_k; }

@@ -77,10 +77,7 @@ def test_sampler_matches_oracle(temperature, top_k, top_p, min_p, rep):
         t_ref, f_ref = Q.sample_token(logits[b], float(u[b]), temperature, top_k, top_p, rep, seen_lists[b], suppress, min_p, return_filtered=True)
         assert int(tok[b]) == t_ref
         if temperature > 0:
-            fb = filt[b].cpu()
-            assert torch.equal(torch.isinf(fb), torch.isinf(f_ref))
-            live = ~torch.isinf(f_ref)
-            assert float((fb[live] - f_ref[live]).abs().max()) < 1e-5
+            assert torch.equal(filt[b].cpu(), f_ref)                     # the scaled logits (logits / temperature) or -inf
 
 
 def _talker(cfg_over, seed=11):

@@ -182,9 +182,11 @@ def test_embedding_is_deterministic(released):
     assert torch.equal(enc(mel), enc(mel))
 
 
-def test_launch_budget_and_no_torch_kernels(released):
+def test_launch_budget_and_no_torch_kernels_in_a_complete_trace(released):
     """One extract_speaker_embedding at B = 1 (3 s of audio): at most 40 launches, and no torch kernel (the samples' host -> device copy
-    is a memcpy)."""
+    is a memcpy).  Every trace the profiler returns is checked for torch kernels.  In a long process it occasionally returns the
+    activity records of earlier work instead of this call's, so a trace without the call's three Res2Net kernels is taken again
+    (up to three times); a pass that stops launching them fails every attempt."""
     from mlx_audio_b200 import ops
     from mlx_audio_b200.tts.models.qwen3_tts import Model, ModelConfig
     enc, _ = released
@@ -193,15 +195,20 @@ def test_launch_budget_and_no_torch_kernels(released):
     audio = (0.3 * np.random.default_rng(3).standard_normal(72000)).astype(np.float32)
     model.extract_speaker_embedding(audio)
     torch.cuda.synchronize()
-    l0 = ops.LAUNCHES[0]
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        model.extract_speaker_embedding(audio)
-        torch.cuda.synchronize()
-    n = ops.LAUNCHES[0] - l0
-    assert n <= 40, n
-    kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and not e.name.startswith(("Memcpy", "Memset"))]
-    assert any("spk_res2net" in k for k in kernels), kernels
-    assert not [k for k in kernels if "at::" in k], kernels
+    traces = []
+    for _ in range(3):
+        l0 = ops.LAUNCHES[0]
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            model.extract_speaker_embedding(audio)
+            torch.cuda.synchronize()
+        n = ops.LAUNCHES[0] - l0
+        assert n <= 40, n
+        kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and not e.name.startswith(("Memcpy", "Memset"))]
+        assert not [k for k in kernels if "at::" in k], kernels
+        traces.append(kernels)
+        if sum("spk_res2net" in k for k in kernels) == 3:
+            break
+    assert sum("spk_res2net" in k for k in traces[-1]) == 3, traces
 
 
 # ---------------------------------------------------------------------------------------------------------------- generation
