@@ -110,11 +110,18 @@ __device__ __forceinline__ TileRef decode_tile(const FParams& p, int tile) {
   return t;
 }
 
-template <typename T> __device__ __forceinline__ T cvt16(float v);
-template <> __device__ __forceinline__ __nv_bfloat16 cvt16<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-template <> __device__ __forceinline__ __half cvt16<__half>(float v) { return __float2half_rn(v); }
-__device__ __forceinline__ float back16(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float back16(__half v) { return __half2float(v); }
+// tc::split16 of two adjacent channels a (low half) and b (high half) with packed conversions: bit-identical to two scalar calls
+template <typename T16> __device__ __forceinline__ void split16x2(float a, float b, uint32_t& hi, uint32_t& lo);
+template <> __device__ __forceinline__ void split16x2<__nv_bfloat16>(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(a - __low2float(h), b - __high2float(h));
+  hi = *reinterpret_cast<const uint32_t*>(&h); lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+template <> __device__ __forceinline__ void split16x2<__half>(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const __half2 l = __floats2half2_rn(a - __low2float(h), b - __high2float(h));
+  hi = *reinterpret_cast<const uint32_t*>(&h); lo = *reinterpret_cast<const uint32_t*>(&l);
+}
 
 __device__ __noinline__ float act_slow(float v, int act, float p0) { return b2a_act(v, act, p0, 1.f, 1.f); }
 __device__ __noinline__ float act_slow2(float v, int act, float p0, float a, float b) { return b2a_act(v, act, p0, a, b); }
@@ -131,28 +138,30 @@ __device__ __forceinline__ void stamp(const FParams& p, int slot) {
 template <typename T16, int ACT>
 __device__ __forceinline__ void convert_store(float4 v, bool valid, const float sc[4], const float sh[4], const float aa[4], const float bb[4],
                                               const bool chok[4], int act, float p0, uint8_t* hi, uint8_t* lo, int r, int c4, bool do_store = true) {
-  float t[4] = {v.x, v.y, v.z, v.w};
-  __align__(8) T16 h[4];
-  __align__(8) T16 l[4];
+  const float t[4] = {v.x, v.y, v.z, v.w};
+  float u[4];
+  // Every element is transformed and the padding / out-of-range ones are replaced by zero afterwards: a branch per element around the
+  // transform cost a BSSY / BSYNC pair each, and the worker warps' instruction issue bounds the generator-stage launches (DESIGN.md §5).
 #pragma unroll
   for (int q = 0; q < 4; q++) {
-    float u = 0.f;
-    if (valid && chok[q]) {
-      u = fmaf(t[q], sc[q], sh[q]);
-      if constexpr (ACT == B2A_ACT_SNAKE) { const float s = b2a_sin_fast(aa[q] * u); u = fmaf(bb[q], s * s, u); }
-      else if constexpr (ACT == B2A_ACT_LRELU) u = u > 0.f ? u : u * p0;
-      else if constexpr (ACT == B2A_ACT_ELU) u = u > 0.f ? u : expm1f(u);
-      else if constexpr (ACT == 0) { }
-      else if (act) u = act_slow2(u, act, p0, aa[q], bb[q]);
-    }
-    h[q] = cvt16<T16>(u);
-    l[q] = cvt16<T16>(u - back16(h[q]));
+    const bool ok = valid && chok[q];
+    float w = fmaf(t[q], sc[q], sh[q]);
+    if constexpr (ACT == B2A_ACT_SNAKE) { const float s = b2a_sin_fast(aa[q] * w); w = fmaf(bb[q], s * s, w); }
+    else if constexpr (ACT == B2A_ACT_LRELU) w = w > 0.f ? w : w * p0;
+    else if constexpr (ACT == B2A_ACT_ELU) w = w > 0.f ? w : expm1f(w);
+    else if constexpr (ACT == 0) { }
+    else if (ok && act) w = act_slow2(w, act, p0, aa[q], bb[q]);
+    u[q] = ok ? w : 0.f;
   }
+  // hi = rn(u), lo = rn(u - hi), two channels per conversion instruction (the same round-to-nearest as the scalar conversions)
+  uint2 h, l;
+  split16x2<T16>(u[0], u[1], h.x, l.x);
+  split16x2<T16>(u[2], u[3], h.y, l.y);
   const uint32_t off = (uint32_t)r * 128u + ((((uint32_t)c4 >> 1) ^ ((uint32_t)r & 7u)) << 4) + (((uint32_t)c4 & 1u) << 3);
   if (do_store) {
-    *reinterpret_cast<uint2*>(hi + off) = *reinterpret_cast<uint2*>(h);
-    if (lo) *reinterpret_cast<uint2*>(lo + off) = *reinterpret_cast<uint2*>(l);
-  } else if (reinterpret_cast<uint2*>(h)->x == 0x12345678u && reinterpret_cast<uint2*>(l)->y == 0x9abcdef0u) {
+    *reinterpret_cast<uint2*>(hi + off) = h;
+    if (lo) *reinterpret_cast<uint2*>(lo + off) = l;
+  } else if (h.x == 0x12345678u && l.y == 0x9abcdef0u) {
     hi[0] = 1;                                                             // timing experiment: keep the conversion alive without the stores
   }
 }
@@ -227,10 +236,15 @@ __device__ __forceinline__ MmaCtl mma_ctl(const FProb& P, const TileRef& t) {
 // A buffer is then handed back.  two_a comes from the kernel parameters (uniform), the rest from MmaCtl.  acc is the caller's one
 // 64-register accumulator, live across the tile loop, of which an NB variant uses the first NB * 16: with a separate array per variant
 // ptxas gives each its own register range (16 + 32 + 48 + 64 = 160 registers) and serialises the wgmmas for want of registers (C7512).
-template <int NB, bool F16>
+// DBG: mwait (shared memory, this warpgroup's leader writes) accumulates the SM cycles spent waiting on full / a_full / tempty and in
+// wgmma.wait_group (MW_* below).  The wait itself is emitted once either way: a second copy of each wgmma.wait_group would double the
+// WARPGROUP.DEPBARs that tests/test_conv_fused_compile.py bounds.
+enum { MW_FULL, MW_AFULL, MW_TEMPTY, MW_WGMMA, MW_N };
+#define MMA_TIMED(slot, stmt) do { if constexpr (DBG) { const long long t0_ = clock64(); stmt; if (leader) mwait[slot] += (unsigned long long)(clock64() - t0_); } else { stmt; } } while (0)
+template <int NB, bool F16, bool DBG>
 __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const MmaCtl& c, bool two_a, float* acc, uint32_t a0, uint32_t w0,
                                          uint64_t* full, uint64_t* empty, uint64_t* a_full, uint64_t* a_empty, uint64_t* tfull, uint64_t* tempty,
-                                         float* acct, uint32_t lt, uint32_t& s, uint32_t& ph, uint32_t& cg) {
+                                         float* acct, uint32_t lt, uint32_t& s, uint32_t& ph, uint32_t& cg, unsigned long long* mwait) {
   const int wg = threadIdx.x >> 7;
   const bool leader = (threadIdx.x & 127) == 0;
   const int kc0 = c.kc0, kc1 = c.kc1;
@@ -241,10 +255,10 @@ __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const
   uint32_t accum = 0;                                            // the tile's first MMA overwrites the accumulator
   for (int kc = kc0; kc < kc1; kc++, cg++) {
     const uint32_t ab = cg & 1;
-    mbar_wait(a_full + ab, (cg >> 1) & 1);
+    MMA_TIMED(MW_AFULL, mbar_wait(a_full + ab, (cg >> 1) & 1));
     const uint32_t abase = a0 + ab * a_buf + (uint32_t)wg * 64u * 128u;
     for (int tap = 0; tap < taps; tap++) {
-      mbar_wait(full + s, ph);
+      MMA_TIMED(MW_FULL, mbar_wait(full + s, ph));
       const uint32_t wa = w0 + s * (uint32_t)p.w_stage;
       const uint32_t aa = abase + (uint32_t)(P.shift[tap] - smin) * 128u;
       const uint64_t wd = gmma_desc_sw128(wa), ad = gmma_desc_sw128(aa);
@@ -254,7 +268,7 @@ __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const
       if (two_a) wgmma_chunk<NB, F16>(acc, gmma_desc_sw128(aa + a_plane), wd, 1u);         // a_lo * w_hi
       if (two_w) wgmma_chunk<NB, F16>(acc, ad, gmma_desc_sw128(wa + wb), 1u);              // a_hi * w_lo
       wgmma_commit();
-      wgmma_wait<1>();
+      MMA_TIMED(MW_WGMMA, wgmma_wait<1>());
       wgmma_fence_regs<NB * 16>(acc);
       if (leader) {
         if (pend_s >= 0) mbar_arrive(empty + pend_s);
@@ -265,13 +279,13 @@ __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const
       if (++s == (uint32_t)p.wst) { s = 0; ph ^= 1; }
     }
   }
-  wgmma_wait<0>();
+  MMA_TIMED(MW_WGMMA, wgmma_wait<0>());
   wgmma_fence_regs<NB * 16>(acc);
   if (leader) {
     if (pend_s >= 0) mbar_arrive(empty + pend_s);
     if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
   }
-  mbar_wait(tempty, (lt & 1) ^ 1);                               // the workers have drained the previous tile
+  MMA_TIMED(MW_TEMPTY, mbar_wait(tempty, (lt & 1) ^ 1));         // the workers have drained the previous tile
   store_acc<NB>(acc, acct, p.acc_ld, wg * 64);
   __syncwarp();
   if ((threadIdx.x & 31) == 0) mbar_arrive(tfull);               // 8 arrivals: the tile is complete
@@ -317,10 +331,12 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
   // inside every role's inner loop (measured: the MMA issuer spent ~1.5 us per K chunk issuing 8 MMAs).  One cooperative copy into shared
   // memory at kernel start makes every later access a ~30-cycle LDS.
   __shared__ __align__(16) FParams sparams;
+  __shared__ unsigned long long mwait_all[DBG ? 2 * MW_N : 1];     // DBG: the MMA warpgroups' wait cycles (see mma_tile)
   {
     const uint32_t* src = reinterpret_cast<const uint32_t*>(&gp);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&sparams);
     for (int i = threadIdx.x; i < (int)(sizeof(FParams) / 4); i += THREADS) dst[i] = src[i];
+    if (DBG && threadIdx.x < 2 * MW_N) mwait_all[threadIdx.x] = 0;
   }
   __syncthreads();
   const FParams& p = sparams;
@@ -390,12 +406,13 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
     float acc[4 * 16];                                          // shared by every NB variant (see mma_tile)
 #pragma unroll
     for (int i = 0; i < 4 * 16; i++) acc[i] = 0.f;
+    unsigned long long* const mwait = mwait_all + (DBG ? wgi * MW_N : 0);
     for (int tile = blockIdx.x; tile < gp.ntiles; tile += gridDim.x, lt++) {
       const TileRef t = decode_tile(p, tile);
       const FProb& P = p.pr[t.g];
       const MmaCtl c = mma_ctl(P, t);
-#define B2A_MMA_TILE(NB) (f16 ? mma_tile<NB, true>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg) \
-                              : mma_tile<NB, false>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg))
+#define B2A_MMA_TILE(NB) (f16 ? mma_tile<NB, true, DBG>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg, mwait) \
+                              : mma_tile<NB, false, DBG>(p, P, c, two_a, acc, a0, w0, full, empty, a_full, a_empty, tfull, tempty, acct, lt, s, ph, cg, mwait))
       switch (c.nb) {
         case 1: B2A_MMA_TILE(1); break;
         case 2: B2A_MMA_TILE(2); break;
@@ -698,6 +715,8 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
   if (threadIdx.x == 0) if (DBG) stamp(p, 12);
   __syncthreads();
   if (threadIdx.x == 0) if (DBG) stamp(p, 13);
+  if (DBG && p.dbg && threadIdx.x < MW_N)                          // slots 26..29: both MMA warpgroups' wait cycles, summed
+    p.dbg[(size_t)blockIdx.x * 32 + 26 + threadIdx.x] = mwait_all[threadIdx.x] + mwait_all[MW_N + threadIdx.x];
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
