@@ -81,6 +81,22 @@ typedef struct {
 int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream);
 int32_t b2a_convtr1d_cl(const b2a_conv1d_t* p, void* stream);
 
+/* kernel of the calling host thread's last successful b2a_conv1d_cl / b2a_convtr1d_cl launch: out[0] = B2A_CONV_PATH_*, out[1..3] its
+ * variant -- narrow: (prologue ACT it was compiled for, -1 = generic, 0, vector staging); dense: (BN, CI, 0); dw_tiled4: (CW, KT,
+ * SNAKE); dw_tiled: (KT, 0, 0); convtr_dense: (BN = 64, CI, 0); the others (0, 0, 0).  All zero before the first launch.  Host-side
+ * record only. */
+enum {
+  B2A_CONV_PATH_LINEAR_ROWS = 1,
+  B2A_CONV_PATH_NARROW = 2,
+  B2A_CONV_PATH_DENSE = 3,
+  B2A_CONV_PATH_DW_TILED4 = 4,
+  B2A_CONV_PATH_DW_TILED = 5,
+  B2A_CONV_PATH_DW = 6,
+  B2A_CONV_PATH_CONVTR_DENSE = 7,
+  B2A_CONV_PATH_CONVTR_DW = 8
+};
+int32_t b2a_conv1d_cl_last_path(int32_t* out4);
+
 /* ---- tensor-core path for dense stride-1 convs / Linears (csrc/gemm_tc.cu) --------------------------------
  * b2a_prep_bf16: the conv prologue (pre_scale/shift + activation, as in b2a_conv1d_t) evaluated once per element and
  * stored as two bf16 planes hi = bf16(v), lo = bf16(v - hi), each [B, L, cpad] (cpad multiple of 64, pad channels zero);

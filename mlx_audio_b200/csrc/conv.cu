@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(NT) conv1d_dw_tiled4_kernel(const b2a_conv1d_t
 // HBM-bound by construction: x is read once, y is 1/Cin of it.
 constexpr int NW_TL = 256;
 template <int ACT>      // ACT >= 0: prologue activation fixed at compile time (no AdaIN scale/shift); -1: generic functor
-__global__ void __launch_bounds__(NT) conv1d_narrow_kernel(const b2a_conv1d_t p, int rows) {
+__global__ void __launch_bounds__(NT) conv1d_narrow_kernel(const b2a_conv1d_t p, int rows, bool v4) {   // v4: 16-byte staging loads
   extern __shared__ __align__(16) float smem[];
   const int ldx = p.Cin + 1;
   float* xs = smem;                                   // [rows][Cin+1]
@@ -267,7 +267,6 @@ __global__ void __launch_bounds__(NT) conv1d_narrow_kernel(const b2a_conv1d_t p,
   };
   const float* xb = p.x + (int64_t)b * p.x_bs;
   const int64_t pos0 = (int64_t)l0 - p.pad_left;
-  const bool v4 = (p.Cin % 4 == 0) && (p.x_ld % 4 == 0) && (p.x_bs % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.x) & 15) == 0);
   if (v4) {
     // 16-byte loads, four in flight per thread before the first is consumed (the scalar one-load-per-iteration loop left the CTA
     // waiting a full memory latency 64 times per tile: 9.7 ms for Mimi's 4.9 GB head instead of ~1 ms)
@@ -557,7 +556,20 @@ __global__ void __launch_bounds__(128) linear_rows_kernel(const b2a_conv1d_t p, 
     }
   }
 }
+
+thread_local int32_t g_last_path[4] = {0, 0, 0, 0};     // kernel id + variant of this host thread's last launch (b2a_conv1d_cl_last_path)
+
+void set_last_path(int32_t kernel, int32_t v1 = 0, int32_t v2 = 0, int32_t v3 = 0) {
+  g_last_path[0] = kernel; g_last_path[1] = v1; g_last_path[2] = v2; g_last_path[3] = v3;
+}
 }  // namespace
+
+/* which kernel instantiation the dispatch rules below chose, so that tests can assert the branch they exercised */
+extern "C" int32_t b2a_conv1d_cl_last_path(int32_t* out4) {
+  B2A_CHECK_ARG(out4, "null pointer");
+  for (int i = 0; i < 4; i++) out4[i] = g_last_path[i];
+  return B2A_OK;
+}
 
 extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
   int bad = check_common(p);
@@ -573,8 +585,10 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
     const int rows = p->B * p->L;
     linear_rows_kernel<<<cdiv(p->Cout, 128), 128, (size_t)rows * p->Cin * sizeof(float), st>>>(*p, rows);
     B2A_CHECK_LAUNCH();
+    set_last_path(B2A_CONV_PATH_LINEAR_ROWS);
     return B2A_OK;
   }
+  int32_t kernel = 0, v1 = 0, v2 = 0, v3 = 0;          // the launch's b2a_conv1d_cl_last_path record
   if (p->groups == 1 && p->stride == 1 && p->Cout <= 4 && p->Lout >= NW_TL &&
       ((size_t)(NW_TL + (p->K - 1) * p->dilation) * (p->Cin + 1) + (size_t)p->K * p->Cin * p->Cout) * sizeof(float) <= 160 * 1024) {
     const int rows = NW_TL + (p->K - 1) * p->dilation;
@@ -589,12 +603,16 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
       attr = true;
     }
     dim3 grid(cdiv(p->Lout, NW_TL), p->B);
-    if (p->pre_scale) conv1d_narrow_kernel<-1><<<grid, NT, sm, st>>>(*p, rows);
-    else if (p->pre_act == 0) conv1d_narrow_kernel<0><<<grid, NT, sm, st>>>(*p, rows);
-    else if (p->pre_act == B2A_ACT_SNAKE && p->pre_a && p->pre_b) conv1d_narrow_kernel<B2A_ACT_SNAKE><<<grid, NT, sm, st>>>(*p, rows);
-    else if (p->pre_act == B2A_ACT_ELU) conv1d_narrow_kernel<B2A_ACT_ELU><<<grid, NT, sm, st>>>(*p, rows);
-    else if (p->pre_act == B2A_ACT_LRELU) conv1d_narrow_kernel<B2A_ACT_LRELU><<<grid, NT, sm, st>>>(*p, rows);
-    else conv1d_narrow_kernel<-1><<<grid, NT, sm, st>>>(*p, rows);
+    const bool v4 = (p->Cin % 4 == 0) && (p->x_ld % 4 == 0) && (p->x_bs % 4 == 0) && (((uintptr_t)p->x & 15) == 0);
+    const int act = p->pre_scale ? -1
+                  : (p->pre_act == 0 || p->pre_act == B2A_ACT_ELU || p->pre_act == B2A_ACT_LRELU ||
+                     (p->pre_act == B2A_ACT_SNAKE && p->pre_a && p->pre_b)) ? p->pre_act : -1;
+    if (act == 0) conv1d_narrow_kernel<0><<<grid, NT, sm, st>>>(*p, rows, v4);
+    else if (act == B2A_ACT_SNAKE) conv1d_narrow_kernel<B2A_ACT_SNAKE><<<grid, NT, sm, st>>>(*p, rows, v4);
+    else if (act == B2A_ACT_ELU) conv1d_narrow_kernel<B2A_ACT_ELU><<<grid, NT, sm, st>>>(*p, rows, v4);
+    else if (act == B2A_ACT_LRELU) conv1d_narrow_kernel<B2A_ACT_LRELU><<<grid, NT, sm, st>>>(*p, rows, v4);
+    else conv1d_narrow_kernel<-1><<<grid, NT, sm, st>>>(*p, rows, v4);
+    kernel = B2A_CONV_PATH_NARROW; v1 = act; v3 = v4;
   } else if (p->groups == 1) {
     const int CI = p->K <= 4 ? 32 : (p->K <= 12 ? 16 : 8);
     const int rows = (BM - 1) * p->stride + (p->K - 1) * p->dilation + 1;
@@ -611,6 +629,7 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
       if (!attr) { cudaFuncSetAttribute(conv1d_dense_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
       conv1d_dense_kernel<16><<<grid, NT, smem, st>>>(*p, CI, rows);
     }
+    kernel = B2A_CONV_PATH_DENSE; v1 = BN; v2 = CI;
   } else if (p->groups == p->Cin && p->Cin == p->Cout) {
     int rows = DW_TL + (p->K - 1) * p->dilation;
     const bool v4 = p->stride == 1 && p->K <= 16 && p->Lout >= DW_TL && p->Cout % 4 == 0 && p->x_ld % 4 == 0 && p->x_bs % 4 == 0 &&
@@ -646,6 +665,7 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
         if (CW == 128) conv1d_dw_tiled4_kernel<0, 128, false><<<grid, NT, sm, st>>>(*p, rows);
         else conv1d_dw_tiled4_kernel<0, 64, false><<<grid, NT, sm, st>>>(*p, rows);
       }
+      kernel = B2A_CONV_PATH_DW_TILED4; v1 = CW; v2 = p->K == 7 ? 7 : 0; v3 = p->K == 7 && snake;
     } else if (p->stride == 1 && p->K <= 16 && rows * 32 * 4 <= 96 * 1024 && p->Lout >= DW_TL) {
       dim3 grid((p->Lout + DW_TL - 1) / DW_TL, (p->Cout + 31) / 32, p->B);
       size_t sm = (size_t)rows * 32 * sizeof(float);
@@ -656,16 +676,19 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
         if (sm > 48 * 1024) cudaFuncSetAttribute(conv1d_dw_tiled_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         conv1d_dw_tiled_kernel<0><<<grid, NT, sm, st>>>(*p, rows);
       }
+      kernel = B2A_CONV_PATH_DW_TILED; v1 = p->K == 7 ? 7 : 0;
     } else {
       int64_t total = (int64_t)p->B * p->Lout * p->Cout;
       int blocks = (int)((total + NT - 1) / NT); if (blocks > 132 * 32) blocks = 132 * 32;
       conv1d_dw_kernel<<<blocks, NT, 0, st>>>(*p);
+      kernel = B2A_CONV_PATH_DW;
     }
   } else {
     b2a_set_error("b2a_conv1d_cl: groups must be 1 or Cin==Cout==groups (got %d)", p->groups);
     return B2A_E_UNSUPPORTED;
   }
   B2A_CHECK_LAUNCH();
+  set_last_path(kernel, v1, v2, v3);
   return B2A_OK;
 }
 
@@ -686,14 +709,17 @@ extern "C" int32_t b2a_convtr1d_cl(const b2a_conv1d_t* p, void* stream) {
     if (!attr) { cudaFuncSetAttribute(convtr1d_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
     dim3 grid(cdiv(p->Lout, BM), cdiv(p->Cout, 64), p->B);
     convtr1d_dense_kernel<<<grid, NT, smem, st>>>(*p, CI, rows, J);
+    B2A_CHECK_LAUNCH();
+    set_last_path(B2A_CONV_PATH_CONVTR_DENSE, 64, CI);
   } else if (p->groups == p->Cin && p->Cin == p->Cout) {
     dim3 grid(cdiv(p->Lout, TRDW_ROWS), cdiv(p->Cout, 128), p->B);
     convtr1d_dw_kernel<<<grid, 128, 0, st>>>(*p);
+    B2A_CHECK_LAUNCH();
+    set_last_path(B2A_CONV_PATH_CONVTR_DW);
   } else {
     b2a_set_error("b2a_convtr1d_cl: groups must be 1 or Cin==Cout==groups (got %d)", p->groups);
     return B2A_E_UNSUPPORTED;
   }
-  B2A_CHECK_LAUNCH();
   return B2A_OK;
 }
 

@@ -373,6 +373,17 @@ def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, 
     return (out, ws) if stats else out
 
 
+CL_PATHS = {1: "linear_rows", 2: "narrow", 3: "dense", 4: "dw_tiled4", 5: "dw_tiled", 6: "dw", 7: "convtr_dense", 8: "convtr_dw"}
+
+
+def conv1d_cl_last_path() -> dict:
+    """Kernel of this host thread's last b2a_conv1d_cl / b2a_convtr1d_cl launch: {"kernel": name (None before any launch),
+    "variant": (v1, v2, v3)} as include/b200audio.h lists them per kernel (dense: (BN, CI, 0), dw_tiled4: (CW, KT, SNAKE), ...)."""
+    out = (C.c_int32 * 4)()
+    _lib.check(_lib.lib().b2a_conv1d_cl_last_path(out))
+    return {"kernel": CL_PATHS.get(out[0]), "variant": (out[1], out[2], out[3])}
+
+
 def conv1d_tc_last_config() -> dict:
     """Tiling of this host thread's last b2a_conv1d_tc launch: {"BN", "grid": (x, y, z), "stages"} (BN 0 before any launch)."""
     out = (C.c_int32 * 5)()
