@@ -428,6 +428,40 @@ typedef struct {
  * any range another entry reads or writes (B2A_E_INVALID otherwise).  Empty entries are skipped. */
 int32_t b2a_stream_rows(const b2a_rowop_t* ops, int32_t n, void* stream);
 
+/* ---- incremental Mimi codec (mimi_stream.cu): Mimi.decode_step / encode_step (codec/models/mimi/mimi.py:164-176) ----------------
+ * b2a_conv1d_stream: StreamableConv1d.step (mimi/modules/conv.py:245-273) -- a causal conv over the virtual input [history | new rows],
+ * history = the H input rows the previous call did not consume.  p->x holds the L new rows (x may be NULL when L == 0), p->Lout must be
+ * the number of complete windows, (H + L - keff) / stride + 1 or 0, keff = (K-1)*dilation + 1, and output row l reads virtual rows
+ * l*stride + k*dilation (p->pad_left is ignored).  Prologue (pre_act, pre_p0), bias, post_act, post_cscale, res / res_div, out_scale as
+ * in b2a_conv1d_t; dense only (groups 1); no pre_scale / shift, Snake, emit or accumulate.  The same launch writes the new history,
+ * virtual rows [Lout*stride, H + L), into the other slot of hist: float [2][B][keff-1][Cin] with batch stride hist_bs (>= (keff-1)*Cin),
+ * slot (*step_dev & 1) being read -- so the caller flips the parity once per step (b2a_stream_advance) and never concatenates.
+ * fresh != 0: the first call of a stream, the history rows are the causal left padding instead -- zeros (pad_mode 0) or the first new
+ * row (pad_mode 1, replicate); a fresh call with L == 0 writes nothing. */
+int32_t b2a_conv1d_stream(const b2a_conv1d_t* p, float* hist, int64_t hist_bs, int32_t H, const int32_t* step_dev, int32_t fresh,
+                          void* stream);
+/* b2a_convtr1d_stream: StreamableConvTranspose1d.step (conv.py:315-331) -- y [B, L*stride, Cout] = bias + the transposed conv of the L new
+ * rows (scatter rule of b2a_convtr1d_cl, no crop) + tail on the first K - stride rows; tail [B, K - stride, Cout] (batch stride tail_bs,
+ * row stride Cout, zero at the start of a stream) is then replaced by output rows [L*stride, L*stride + K - stride) WITHOUT the bias (the
+ * reference subtracts it).  Dense or depthwise (groups == Cin == Cout); prologue activation, bias and out_scale only; K - stride <= L*stride. */
+int32_t b2a_convtr1d_stream(const b2a_conv1d_t* p, float* tail, int64_t tail_bs, void* stream);
+/* Windowed attention over a ring KV cache (transformer.py:79-112 with the growing KVCache and the context mask), position counter on the
+ * device so that a captured step replays without host scalars:
+ * b2a_ring_rope_kv: qkv [B, T, 3 H D] ([q | k | v], head h at +h*D, token stride qkv_ld): interleaved-pair RoPE (nn.RoPE traditional, base)
+ *   of q (in place) and k at absolute positions *pos_dev + t; rotated k and v stored at ring row (*pos_dev + t) % cap of k_ring / v_ring
+ *   [B, cap, H D] (batch stride ring_bs).
+ * b2a_ring_attn: out[b, t, h] = softmax(scale q k^T) v over the ring positions [max(0, p - window + 1), p], p = *pos_dev + t (keys in
+ *   ascending position order, fixed reduction trees: bit-reproducible); q [B, T, H D] rows (the rotated q of b2a_ring_rope_kv).  D == 64,
+ *   window <= 1024, cap >= window + T - 1 (a new row never overwrites a key some query of the call still sees), 16-byte aligned ring rows.
+ *   Neither advances the counter. */
+int32_t b2a_ring_rope_kv(float* qkv, int64_t qkv_bs, int64_t qkv_ld, int32_t B, int32_t T, int32_t H, int32_t D, float base,
+                         float* k_ring, float* v_ring, int64_t ring_bs, int32_t cap, const int32_t* pos_dev, void* stream);
+int32_t b2a_ring_attn(const float* q, int64_t q_bs, int64_t q_ld, const float* k_ring, const float* v_ring, int64_t ring_bs, int32_t cap,
+                      float* out, int64_t o_bs, int64_t o_ld, int32_t B, int32_t T, int32_t H, int32_t D, float scale, int32_t window,
+                      const int32_t* pos_dev, void* stream);
+/* End of a streaming step: ctr[0] (ring position) += dpos, ctr[1] (history slot parity counter) += 1. */
+int32_t b2a_stream_advance(int32_t* ctr, int32_t dpos, void* stream);
+
 /* ---- Qwen3-TTS speaker encoder (ECAPA-TDNN, tts/models/qwen3_tts/speaker_encoder.py) and its log-mel front end -------------- */
 /* qwen3_tts.py:64-121 (mel_spectrogram): reflect pad of (1024-256)/2 samples (no repeated edge), STFT (n_fft 1024, hop 256,
  * center=False, periodic Hann `window`), sqrt(|X|^2 + 1e-9) @ filters^T (Slaney mel, [n_mels, 513]), log(max(., 1e-5)).

@@ -128,6 +128,11 @@ PROTOTYPES = {
     "b2a_snac_from_codes": (i32, [C.POINTER(C.c_void_p), C.POINTER(i32), i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                   C.POINTER(C.c_void_p), i32, i64, i32, i32, i32, c_f, c_f, C.c_void_p]),
     "b2a_stream_rows": (i32, [C.POINTER(RowOp), i32, C.c_void_p]),
+    "b2a_conv1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, i32, c_f, i32, C.c_void_p]),
+    "b2a_convtr1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, C.c_void_p]),
+    "b2a_ring_rope_kv": (i32, [c_f, i64, i64, i32, i32, i32, i32, f32, c_f, c_f, i64, i32, c_f, C.c_void_p]),
+    "b2a_ring_attn": (i32, [c_f, i64, i64, c_f, c_f, i64, i32, c_f, i64, i64, i32, i32, i32, i32, f32, i32, c_f, C.c_void_p]),
+    "b2a_stream_advance": (i32, [c_f, i32, C.c_void_p]),
     "b2a_spk_logmel": (i32, [c_f, i64, i32, i64, c_f, c_f, i32, i64, c_f, C.c_void_p]),
     "b2a_spk_reflect_pad": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, c_f, i32, C.c_void_p]),
     "b2a_spk_res2net_smem_bytes": (i64, [i32, i32, i32, i32, i32]),

@@ -49,7 +49,10 @@ class Mimi:
         self.cfg = cfg
         self.device = torch.device(device)
         self._w = None
-        self._stream_codes = None
+        self._enc = None
+        self._states = {}
+        self._dec_state = None
+        self._enc_state = None
 
     @property
     def frame_rate(self):
@@ -60,23 +63,52 @@ class Mimi:
         return self.cfg.sample_rate
 
     def reset_state(self):
-        """mimi.py:138-144: forget the streaming state."""
-        self._stream_codes = None
+        """mimi.py:138-144: forget the streaming state of both directions."""
+        self._dec_state = None
+        self._enc_state = None
 
     @torch.no_grad()
     def decode_step(self, xs: torch.Tensor) -> torch.Tensor:
-        """mimi.py:171-176: the next ``T_new`` code frames [B, nq, T_new] -> their 1920 T_new samples.  In the reference the incremental
-        path (conv buffers, overlap-add with the bias handled, rotating KV cache) returns exactly the corresponding slice of a one-shot
-        decode (7e-16 when its own code is run, tests/golden/make_codec_golden.py); here the codes seen so far are kept and re-decoded --
-        the same samples, with the cost of a full decode per call (a 10 000-frame decode is 34 ms).  ``reset_state()`` / ``decode()`` start a
-        new stream, as they do in the reference."""
+        """mimi.py:171-176: the next ``T_new`` code frames [B, nq, T_new] -> their samples [B, 1, 1920 T_new], exactly the matching slice of a
+        one-shot ``decode`` of the whole stream for any chunking.  Incremental: every causal conv carries its unconsumed input rows, every
+        transposed conv its held-back tail, the transformer a ring KV cache of ``context`` + chunk positions -- the cost of a call does not
+        depend on how far into the stream it is and memory stays bounded.  Single-frame steps replay a CUDA graph captured once per batch
+        size.  ``reset_state()`` / ``decode()`` start a new stream; the batch size is fixed at the first step after that."""
         xs = xs.to(device=self.device, dtype=torch.int64)
-        prev = getattr(self, "_stream_codes", None)
-        codes = xs if prev is None else torch.cat([prev, xs], dim=-1)
-        pcm = self.decode(codes)
-        self._stream_codes = codes
-        hop = pcm.shape[-1] // codes.shape[-1]
-        return pcm[..., (codes.shape[-1] - xs.shape[-1]) * hop:]
+        if xs.dim() != 3 or not 1 <= xs.shape[1] <= self.cfg.nq:
+            raise ValueError(f"decode_step: expected codes [B, <= {self.cfg.nq}, T], got {tuple(xs.shape)}")
+        st = self._dec_state
+        if st is None:
+            st = self._dec_state = self._state("dec", xs.shape[0])
+        elif xs.shape[0] != st.B:
+            raise ValueError(f"decode_step: batch size {xs.shape[0]} differs from the stream's {st.B} (reset_state() starts a new stream)")
+        return st.decode(xs)
+
+    @torch.no_grad()
+    def encode_step(self, xs: torch.Tensor) -> torch.Tensor:
+        """mimi.py:164-169: the next ``n`` samples pcm [B, 1, n] -> int64 codes [B, nq, F] of the F frames this call completes (possibly 0);
+        leftover samples are carried.  Over a stream the codes equal ``encode`` of the concatenated audio (for audio ending on a frame
+        boundary).  ``reset_state()`` / ``encode()`` start a new stream; the batch size is fixed at the first step after that."""
+        if self._enc is None:
+            raise ValueError("Mimi.encode_step: the loaded weights have no encoder (encoder.*, encoder_transformer.*, downsample.*)")
+        xs = xs.to(device=self.device, dtype=torch.float32)
+        if xs.dim() != 3 or xs.shape[1] != 1:
+            raise ValueError(f"encode_step: expected pcm [B, 1, n], got {tuple(xs.shape)}")
+        st = self._enc_state
+        if st is None:
+            st = self._enc_state = self._state("enc", xs.shape[0])
+        elif xs.shape[0] != st.B:
+            raise ValueError(f"encode_step: batch size {xs.shape[0]} differs from the stream's {st.B} (reset_state() starts a new stream)")
+        return st.encode(xs)
+
+    def _state(self, direction: str, B: int) -> "MimiStreamState":
+        """The (B, direction) state: allocated once, zeroed in place for every new stream (a captured graph keeps its buffers)."""
+        key = (direction, B)
+        st = self._states.get(key)
+        if st is None:
+            st = self._states[key] = MimiStreamState(self, direction, B)
+        st.reset()
+        return st
 
     @property
     def span_halo(self) -> int:
@@ -187,6 +219,8 @@ class Mimi:
         del bf
         self._w = W
         self._enc = None
+        self._states = {}
+        self.reset_state()
         if "encoder.init_conv1d.conv.conv.weight" in P:                 # encode side (seanet.py:194-199, mimi.py:146-153, quantization.py:178-185)
             self._enc = load_encoder(P, cfg, dev, W["cb_first"], W["cb_rest"])
         return self
@@ -195,7 +229,7 @@ class Mimi:
     def decode(self, codes: torch.Tensor) -> torch.Tensor:
         """codes int64 [B, nq, T] -> pcm [B, 1, 1920 T]."""
         W, cfg, dev = self._w, self.cfg, self.device
-        self._stream_codes = None                                       # decode() resets the streaming state (mimi.py:156-158)
+        self._dec_state = None                                          # decode() resets the decode stream (mimi.py:156-158)
         codes = codes.to(device=dev, dtype=torch.int64).contiguous()
         B, nq, T = codes.shape
         q = ops.rvq_decode(codes[:, :1], W["cb_first"])
@@ -231,6 +265,7 @@ class Mimi:
         """mimi.py:146-153: pcm [B, 1, n] -> int64 codes [B, nq, ceil(n / 1920)]: SEANet encoder, encoder transformer, stride-2 replicate-padded
         down-sampling conv, then the split residual quantiser (quantization.py:178-185): the first codebook on its own projection, the other
         nq - 1 as a residual chain on theirs -- `rvq_encode_kernel` runs the chain (argmin |e|^2 / 2 - x.e, first index on ties)."""
+        self._enc_state = None                                          # encode() resets the encode stream (mimi.py:147-149)
         return encode_codes(self._enc, self.encode_latent(xs))
 
 
@@ -325,6 +360,172 @@ def encode_codes(E: dict, z: torch.Tensor, n_books=None) -> torch.Tensor:
         r2 = ops.conv1d(z, E["in_rest"])
         codes.append(ops.rvq_encode(r2.reshape(B * T, -1), E["cb_rest"][:n_rest], E["c2_rest"][:n_rest]).reshape(B, T, -1))
     return torch.cat(codes, dim=2).transpose(1, 2).contiguous()
+
+
+# ------------------------------------------------------------------------------------------------------------------- streaming
+STREAM_PIECE_FRAMES = 128     # a longer call runs in pieces of this many frames: bounds the ring (context + 2 x 128 positions) and activations
+
+
+def _stream_transformer(x: torch.Tensor, layers, cfg: MimiConfig, k_ring, v_ring, ctr: torch.Tensor) -> torch.Tensor:
+    """``_transformer`` for the next positions of a stream: RoPE at the absolute positions ctr[0] + t, k / v into each layer's ring, the
+    ``cfg.context`` window over the ring (transformer.py:79-112 with a growing KVCache)."""
+    d, nh = cfg.dimension, cfg.num_heads
+    for lw, kr, vr in zip(layers, k_ring, v_ring):
+        n1 = ops.layernorm(x, *lw["n1"], eps=1e-5)
+        qkv = ops.linear(n1, lw["in_proj"])
+        ops.ring_rope_kv(qkv, nh, kr, vr, ctr, base=cfg.max_period)
+        att = ops.ring_attn(qkv[:, :, :d], kr, vr, ctr, n_heads=nh, scale=(d // nh) ** -0.5, window=cfg.context)
+        x = ops.linear(att, lw["out_proj"], cscale=lw["ls1"], res=x)
+        n2 = ops.layernorm(x, *lw["n2"], eps=1e-5)
+        m = ops.linear(n2, lw["l1"], post_act=ACT["gelu_tanh"])
+        x = ops.linear(m, lw["l2"], cscale=lw["ls2"], res=x)
+    return x
+
+
+class MimiStreamState:
+    """Device state of one streaming direction ("dec" or "enc") at batch size B, allocated once and zeroed in place by ``reset``:
+    ``ctr`` int32 [ring position, history parity counter], per causal conv a two-slot history [2, B, keff - 1, Cin], per transposed conv
+    its held-back tail [B, K - stride, Cout], per transformer layer a k and a v ring [B, context + 2 x STREAM_PIECE_FRAMES + 2, 512].
+    Decode: single-frame steps replay a CUDA graph captured at the second such step (the first runs eagerly and creates any workspaces).
+    Encode: the histories of the strided convs vary in length (tracked here); transformer positions are processed in whole frames, an odd
+    one waits in ``pend``."""
+
+    def __init__(self, mimi: "Mimi", direction: str, B: int):
+        cfg, dev = mimi.cfg, mimi.device
+        self.m, self.dir, self.B = mimi, direction, B
+        z = lambda *shape: torch.zeros(*shape, device=dev, dtype=torch.float32)
+        hist = lambda cw: z(2, B, max(cw.K - 1, 1), cw.cin)
+        s, d = cfg.upsample_stride, cfg.dimension
+        self.ctr = torch.zeros(2, device=dev, dtype=torch.int32)
+        self.err = torch.zeros(1, device=dev, dtype=torch.int32)
+        self.cap = cfg.context + s * STREAM_PIECE_FRAMES + s
+        self.k_ring = [z(B, self.cap, d) for _ in range(cfg.num_layers)]
+        self.v_ring = [z(B, self.cap, d) for _ in range(cfg.num_layers)]
+        self.bufs = [self.ctr, self.err]
+        if direction == "dec":
+            W = mimi._w
+            self.up_tail = z(B, W["upsample"].K - s, d)
+            self.h_init, self.h_final = hist(W["init"]), hist(W["final"])
+            self.dec = [{"tail": z(B, lw["up"].K - lw["r"], lw["up"].cout), "h0": hist(lw["c0"])} for lw in W["dec"]]
+            self.bufs += [self.up_tail, self.h_init, self.h_final] + [t for sl in self.dec for t in sl.values()]
+            self.graphs = {}              # nq -> (graph, static codes [B, nq, 1], static pcm)
+            self.eager_single = 0
+        else:
+            E = mimi._enc
+            self.convs = {"init": (E["init"], 1)}
+            for i, lw in enumerate(E["layers"]):
+                self.convs[f"c0_{i}"] = (lw["c0"], 1)
+                self.convs[f"down_{i}"] = (lw["down"], lw["r"])
+            self.convs["final"] = (E["final"], 1)
+            self.convs["ds"] = (E["down"], s)
+            self.hist = {k: hist(cw) for k, (cw, _) in self.convs.items()}
+            self.pend = z(B, s, d)
+            self.bufs += list(self.hist.values()) + [self.pend]
+
+    def reset(self):
+        for t in self.bufs:
+            t.zero_()
+        if self.dir == "enc":
+            self.H = {k: cw.K - st for k, (cw, st) in self.convs.items()}        # the causal left padding (fresh: zeros / edge rows)
+            self.fresh = {k: True for k in self.convs}
+            self.npend = 0
+
+    def _check(self):
+        if int(self.err.item()) != 0:
+            raise ValueError(f"decode_step: code index out of range [0, {self.m.cfg.bins})")
+
+    # ---- decode
+    def _decode_piece(self, codes: torch.Tensor) -> torch.Tensor:
+        W, cfg = self.m._w, self.m.cfg
+        B, nq, T = codes.shape
+        q = ops.rvq_decode(codes[:, :1], W["cb_first"], check=False, err=self.err)
+        x = ops.conv1d(q, W["proj_first"])
+        if nq > 1:
+            q2 = ops.rvq_decode(codes[:, 1:], W["cb_rest"][: nq - 1], check=False, err=self.err)
+            x = ops.conv1d(q2, W["proj_rest"], res=x)
+        s = cfg.upsample_stride
+        x = ops.convtr1d_stream(x, W["upsample"], self.up_tail, stride=s)
+        x = _stream_transformer(x, W["layers"], cfg, self.k_ring, self.v_ring, self.ctr)
+        elu, step = Pre(act=ACT["elu"]), self.ctr[1:]
+        x = ops.conv1d_stream(x, W["init"], self.h_init, cfg.ksize - 1, step)
+        for lw, sl in zip(W["dec"], self.dec):
+            y = ops.convtr1d_stream(x, lw["up"], sl["tail"], stride=lw["r"], pre=elu)
+            t = ops.conv1d_stream(y, lw["c0"], sl["h0"], cfg.residual_ksize - 1, step, pre=elu)
+            x = ops.conv1d(t, lw["c1"], pre=elu, res=y)
+        pcm = ops.conv1d_stream(x, W["final"], self.h_final, cfg.last_ksize - 1, step, pre=elu)
+        ops.stream_advance(self.ctr, s * T)
+        return pcm.reshape(B, 1, -1)
+
+    def decode(self, codes: torch.Tensor) -> torch.Tensor:
+        B, nq, T = codes.shape
+        if T == 0:
+            return torch.zeros(B, 1, 0, device=codes.device, dtype=torch.float32)
+        if T == 1 and GRAPH_SINGLE_FRAME[0]:
+            ent = self.graphs.get(nq)
+            if ent is None and self.eager_single > 0:
+                cin = codes.contiguous().clone()
+                torch.cuda.synchronize(codes.device)
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    out = self._decode_piece(cin)
+                ent = self.graphs[nq] = (g, cin, out)
+            if ent is not None:
+                g, cin, out = ent
+                cin.copy_(codes)
+                g.replay()
+                self._check()
+                return out.clone()
+            self.eager_single += 1
+        codes = codes.contiguous()
+        parts = [self._decode_piece(codes[:, :, a:a + STREAM_PIECE_FRAMES].contiguous()) for a in range(0, T, STREAM_PIECE_FRAMES)]
+        self._check()
+        return parts[0] if len(parts) == 1 else torch.cat(parts, dim=-1)
+
+    # ---- encode
+    def _conv(self, name: str, x, pre=None, res=None, pad_mode=0):
+        cw, stride = self.convs[name]
+        L = 0 if x is None else x.shape[1]
+        y = ops.conv1d_stream(x if L else None, cw, self.hist[name], self.H[name], self.ctr[1:], B=self.B, stride=stride, pad_mode=pad_mode,
+                              fresh=self.fresh[name], pre=pre, res=res)
+        if not (self.fresh[name] and L == 0):
+            self.H[name] += L - y.shape[1] * stride
+            self.fresh[name] = False
+        return y
+
+    def _encode_piece(self, pcm: torch.Tensor) -> torch.Tensor:
+        E, cfg, B = self.m._enc, self.m.cfg, self.B
+        elu, s = Pre(act=ACT["elu"]), cfg.upsample_stride
+        x = self._conv("init", pcm.reshape(B, -1, 1).contiguous())
+        for i, lw in enumerate(E["layers"]):
+            t = self._conv(f"c0_{i}", x, pre=elu)
+            y = ops.conv1d(t, lw["c1"], pre=elu, res=x) if t.shape[1] else t.new_zeros(B, 0, x.shape[2])   # block(x) + x (seanet.py:61-66)
+            x = self._conv(f"down_{i}", y, pre=elu)
+        x = self._conv("final", x, pre=elu)
+        n = self.npend + x.shape[1]
+        run = n - n % s                                               # positions that complete frames
+        if run == 0:                                                  # no frame: keep the positions, no transformer launch
+            if x.shape[1]:
+                self.pend[:, self.npend:n].copy_(x)
+            self.npend = n
+            self._conv("ds", None, pad_mode=1)                        # carries the down-sampler's history to the next parity slot
+            ops.stream_advance(self.ctr, 0)
+            return torch.zeros(B, cfg.nq, 0, device=x.device, dtype=torch.int64)
+        z = torch.cat([self.pend[:, :self.npend], x], dim=1) if self.npend else x
+        if n > run:
+            self.pend[:, :n - run].copy_(z[:, run:])
+        self.npend = n - run
+        z = _stream_transformer(z[:, :run].contiguous(), E["tr"], cfg, self.k_ring, self.v_ring, self.ctr)
+        lat = self._conv("ds", z, pad_mode=1)
+        ops.stream_advance(self.ctr, run)
+        return encode_codes(E, lat)
+
+    def encode(self, pcm: torch.Tensor) -> torch.Tensor:
+        n, hop = pcm.shape[-1], STREAM_PIECE_FRAMES * int(round(self.m.cfg.sample_rate / self.m.cfg.frame_rate))
+        parts = [self._encode_piece(pcm[:, :, a:a + hop]) for a in range(0, max(n, 1), hop)] if n else [self._encode_piece(pcm)]
+        return parts[0] if len(parts) == 1 else torch.cat(parts, dim=2)
+
+
+GRAPH_SINGLE_FRAME = [True]      # single-frame decode steps through a captured CUDA graph (False: always eager)
 
 
 class MimiStreamingDecoder:

@@ -639,6 +639,89 @@ def stream_rows(entries) -> None:
     _call("other", _lib.lib().b2a_stream_rows, 1, arr, len(entries), _stream())
 
 
+def _stream_conv_params(x, cw: ConvW, B: int, L: int, lout: int, out, stride: int, dilation: int, pad_mode: int, pre: Optional[Pre],
+                        post_act: int, res, res_div: int) -> Conv1dParams:
+    p = Conv1dParams()
+    if L:
+        _chk3(x, "stream conv x")
+        p.x, p.x_bs, p.x_ld = x.data_ptr(), x.stride(0), x.stride(1)
+    p.B, p.L, p.Cin = B, L, cw.cin
+    p.w, p.bias = cw.w.data_ptr(), _p(cw.bias)
+    if lout:
+        p.y, p.y_bs, p.y_ld = out.data_ptr(), out.stride(0), out.stride(1)
+    p.Lout, p.Cout = lout, cw.cout
+    p.K, p.stride, p.dilation, p.groups, p.pad_mode = cw.K, stride, dilation, cw.groups, pad_mode
+    if pre is not None:
+        if pre.scale is not None or pre.shift is not None or pre.a is not None or pre.b is not None:
+            raise ValueError("stream conv: the prologue is an activation only")
+        p.pre_act, p.pre_p0 = pre.act, pre.p0
+    p.post_act = post_act
+    if res is not None:
+        _chk3(res, "stream conv res")
+        p.res, p.res_bs, p.res_ld = res.data_ptr(), res.stride(0), res.stride(1)
+    p.res_div, p.out_scale = res_div, 1.0
+    return p
+
+
+def conv1d_stream(x: Optional[torch.Tensor], cw: ConvW, hist: torch.Tensor, H: int, step: torch.Tensor, *, B=None, stride=1, dilation=1,
+                  pad_mode=0, fresh=False, pre: Optional[Pre] = None, post_act=0, res=None, res_div=1, out=None) -> torch.Tensor:
+    """b2a_conv1d_stream: the causal conv of [history (H rows) | x] -> its complete windows [B, Lout, Cout] (possibly 0 rows), the unconsumed
+    rows carried into the other slot of ``hist`` float32 [2, B, keff - 1, Cin] (slot ``step[0] & 1`` is read).  ``x`` None = no new rows.
+    Returns the output; the caller's new history length is H + L - Lout * stride."""
+    L = 0 if x is None else x.shape[1]
+    B = x.shape[0] if x is not None else B
+    keff = (cw.K - 1) * dilation + 1
+    lout = (H + L - keff) // stride + 1 if H + L >= keff else 0
+    if hist.dtype != torch.float32 or not hist.is_contiguous() or hist.shape != (2, B, max(keff - 1, 1), cw.cin):
+        raise ValueError(f"conv1d_stream: history buffer must be float32 [2, {B}, {max(keff - 1, 1)}, {cw.cin}], got {tuple(hist.shape)}")
+    if out is None:
+        out = torch.empty(B, lout, cw.cout, device=hist.device, dtype=torch.float32)
+    p = _stream_conv_params(x, cw, B, L, lout, out, stride, dilation, pad_mode, pre, post_act, res, res_div)
+    _call("conv", _lib.lib().b2a_conv1d_stream, 1, C.byref(p), hist.data_ptr(), hist.stride(1), H, step.data_ptr(), int(fresh), _stream())
+    return out
+
+
+def convtr1d_stream(x: torch.Tensor, cw: ConvW, tail: torch.Tensor, *, stride: int, pre: Optional[Pre] = None, out=None) -> torch.Tensor:
+    """b2a_convtr1d_stream: [B, L*stride, Cout] = bias + transposed conv of x + the held-back ``tail`` float32 [B, K - stride, Cout] on the
+    first rows; ``tail`` then holds the next K - stride rows without the bias."""
+    _chk3(x, "convtr1d_stream x")
+    B, L, _ = x.shape
+    if not tail.is_contiguous() or tail.shape != (B, cw.K - stride, cw.cout):
+        raise ValueError(f"convtr1d_stream: tail must be contiguous [{B}, {cw.K - stride}, {cw.cout}], got {tuple(tail.shape)}")
+    if out is None:
+        out = torch.empty(B, L * stride, cw.cout, device=x.device, dtype=torch.float32)
+    p = _stream_conv_params(x, cw, B, L, L * stride, out, stride, 1, 0, pre, 0, None, 1)
+    _call("conv", _lib.lib().b2a_convtr1d_stream, 1, C.byref(p), tail.data_ptr(), tail.stride(0), _stream())
+    return out
+
+
+def ring_rope_kv(qkv: torch.Tensor, n_heads: int, k_ring: torch.Tensor, v_ring: torch.Tensor, pos: torch.Tensor, *, base: float) -> None:
+    """b2a_ring_rope_kv: RoPE (interleaved pairs) of q in place and of k at positions pos[0] + t; k, v into ring rows (pos[0] + t) % cap."""
+    _chk3(qkv, "ring_rope_kv qkv")
+    B, T, w = qkv.shape
+    D = w // (3 * n_heads)
+    _call("rope", _lib.lib().b2a_ring_rope_kv, 1, qkv.data_ptr(), qkv.stride(0), qkv.stride(1), B, T, n_heads, D, base, k_ring.data_ptr(),
+          v_ring.data_ptr(), k_ring.stride(0), k_ring.shape[1], pos.data_ptr(), _stream())
+
+
+def ring_attn(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, pos: torch.Tensor, *, n_heads: int, scale: float, window: int,
+              out=None) -> torch.Tensor:
+    """b2a_ring_attn: q [B, T, H D] (row-strided view) at positions pos[0] + t against the ring caches [B, cap, H D] -> [B, T, H D]."""
+    _chk3(q, "ring_attn q")
+    B, T, hd = q.shape
+    if out is None:
+        out = torch.empty(B, T, hd, device=q.device, dtype=torch.float32)
+    _call("attention", _lib.lib().b2a_ring_attn, 1, q.data_ptr(), q.stride(0), q.stride(1), k_ring.data_ptr(), v_ring.data_ptr(), k_ring.stride(0),
+          k_ring.shape[1], out.data_ptr(), out.stride(0), out.stride(1), B, T, n_heads, hd // n_heads, scale, window, pos.data_ptr(), _stream())
+    return out
+
+
+def stream_advance(ctr: torch.Tensor, dpos: int) -> None:
+    """ctr int32 [2]: ring position += dpos, history parity counter += 1 (the last launch of a streaming step)."""
+    assert ctr.dtype == torch.int32 and ctr.numel() >= 2
+    _call("other", _lib.lib().b2a_stream_advance, 1, ctr.data_ptr(), dpos, _stream())
+
+
 def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor] = None, add: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[r, :] = src[idx[r], :] (+ add[r % add.shape[0], :]); src [N, C] float32, idx int64 [R]."""
     assert src.dim() == 2 and src.stride(1) == 1 and idx.dtype == torch.int64 and idx.is_contiguous()
