@@ -126,6 +126,31 @@ int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16, int32_t B
  * The N tile is the widest divisor of Cout up to 128 unless that grid covers under half the SMs; then the widest whose grid still
  * covers them all (or 32).  Launched with programmatic dependent launch: weight tiles are fetched before the dependency wait. */
 
+/* ---- Kokoro's ALBERT encoder layers in one persistent launch (csrc/albert.cu) -------------------------------
+ * num_hidden_layers passes of the shared AlbertLayer (modules.py:497-560: qkv projection, attention, attn_out + residual, LayerNorm,
+ * ffn + GELU, ffn_out + residual, LayerNorm) over h [T, hidden] fp32, in place, B = 1, 64 <= T <= 512, hidden = 64 * heads.  Inputs:
+ * h and its bf16 planes h_hi / h_lo [T, hidden] (what b2a_layernorm / b2a_conv1d_tc emit; h_lo NULL when planes == 1); both are
+ * overwritten.  Weights as for b2a_conv1d_tc: bf16 [N][K] in the order qkv [3 hidden][hidden], attn_out [hidden][hidden],
+ * ffn [inter][hidden], ffn_out [hidden][inter]; ln_* = (attention LayerNorm, full-layer LayerNorm); scale = the softmax scale.
+ * Every element is computed as b2a_conv1d_tc(planes / attention-operand epilogue), b2a_attention_tc(operands_ready) and
+ * b2a_layernorm(planes) compute it, so the result equals that launch sequence bit for bit. */
+typedef struct {
+  int32_t T, layers, heads, hidden, inter, planes;
+  const void* w[4];
+  const float* bias[4];
+  const float* ln_w[2];
+  const float* ln_b[2];
+  float eps, scale;
+  float* h; void* h_hi; void* h_lo;
+} b2a_albert_t;
+/* bytes of the workspace b2a_albert_encoder needs (256-byte aligned; its first word is the launch's grid barrier, reset by a memset
+ * in front of the kernel) */
+int64_t b2a_albert_ws_bytes(int32_t T, int32_t heads, int32_t hidden, int32_t inter);
+/* One cooperative launch of one CTA per SM.  err: a device word that a grid barrier which sees no progress for 10 s sets to 1 (the
+ * output is then invalid); it is never cleared here.  timeline: NULL, or int64 [layers * 7][SM count][2] that a timeline build of the
+ * kernel fills with globaltimer (ns) at the start and end of every stage of every CTA (profiling). */
+int32_t b2a_albert_encoder(const b2a_albert_t* a, void* ws, uint32_t* err, int64_t* timeline, void* stream);
+
 /* profiling aid: CTA (0,0,0) of subsequent b2a_conv1d_tc launches stamps clock64() at its phase boundaries into dbg8[0..6]
  * (entry, setup done, first operands landed, last operands landed, accumulator ready, epilogue done, exit); NULL disables. */
 int32_t b2a_conv1d_tc_debug(void* dbg8);

@@ -61,6 +61,13 @@ class ConvFParams(C.Structure):
     ]
 
 
+class AlbertParams(C.Structure):
+    """b2a_albert_t"""
+    _fields_ = [("T", i32), ("layers", i32), ("heads", i32), ("hidden", i32), ("inter", i32), ("planes", i32),
+                ("w", C.c_void_p * 4), ("bias", C.c_void_p * 4), ("ln_w", C.c_void_p * 2), ("ln_b", C.c_void_p * 2),
+                ("eps", f32), ("scale", f32), ("h", C.c_void_p), ("h_hi", C.c_void_p), ("h_lo", C.c_void_p)]
+
+
 class RowOp(C.Structure):
     """Mirror of b2a_rowop_t."""
     _fields_ = [("src", C.c_void_p), ("src_bs", i64), ("src_ld", i64), ("dst", C.c_void_p), ("dst_bs", i64), ("dst_ld", i64),
@@ -98,6 +105,8 @@ PROTOTYPES = {
     "b2a_attention": (i32, [C.POINTER(AttnParams), C.c_void_p]),
     "b2a_attention_tc_ws_bytes": (i64, [i32, i32, i32, i32]),
     "b2a_attention_tc": (i32, [C.POINTER(AttnParams), C.c_void_p, C.c_void_p]),
+    "b2a_albert_ws_bytes": (i64, [i32, i32, i32, i32]),
+    "b2a_albert_encoder": (i32, [C.POINTER(AlbertParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2a_rope": (i32, [c_f, i64, i64, i32, i32, i32, i32, i32, f32, i32, C.c_void_p]),
     "b2a_lstm_bidir": (i32, [c_f, c_f, c_f, i64, i32, i32, i32, C.c_void_p]),
     "b2a_stft": (i32, [c_f, i64, i32, i64, c_f, i32, i32, i32, i64, c_f, c_f, C.c_void_p]),

@@ -18,6 +18,7 @@
 // tile per CTA; BN <= 128 keeps the accumulator at <= 64 registers per thread.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "tc_epilogue.cuh"
 #include <stdlib.h>
 
 using namespace tc;
@@ -28,8 +29,6 @@ constexpr int TM = 128;            // rows (positions) per CTA tile = two wgmma 
 constexpr int TK = 64;             // bf16 elements per 128-byte swizzle row == K extent of one stage
 constexpr int THREADS = 288;
 constexpr int BN_MAX = 128;
-
-__device__ __noinline__ float act_noinline(float v, int act, float p0) { return b2a_act(v, act, p0, 1.f, 1.f); }
 
 struct TcParams {
   int B, L, Lout, Cout, cin_pad, taps, planes, wplanes, BN, stages, f16;
@@ -49,34 +48,15 @@ struct TcParams {
   AttnOperands attn; int a_H, a_hs; float a_qmul;
 };
 
-// Where this lane's column of the output tile goes as split16 planes: hi / lo pointers at row 0 of batch b, and the element step per row.
-struct EmitCol { uint16_t *hi, *lo; int64_t step; float mul; bool f16; };
+// Where this lane's column of the output tile goes as split16 planes (tc::EmitCol).
 __device__ __forceinline__ EmitCol emit_col(const TcParams& p, int b, int n) {
+  if (p.attn.qh) return emit_col_attn(p.attn, (int64_t)b * p.a_H, p.Lout, p.a_hs, p.a_qmul, n);
   EmitCol c{nullptr, nullptr, 0, 1.f, false};
-  if (p.attn.qh) {
-    const int part = n / p.a_hs, head = (n - part * p.a_hs) >> 6, d = n & 63;
-    const int64_t bh = (int64_t)b * p.a_H + head;
-    c.f16 = true;
-    if (part < 2) {
-      const int64_t o = bh * p.Lout * 64 + d;
-      c.hi = (uint16_t*)(part ? p.attn.kh : p.attn.qh) + o; c.lo = (uint16_t*)(part ? p.attn.kl : p.attn.ql) + o;
-      c.step = 64; c.mul = part ? 1.f : p.a_qmul;
-    } else {
-      const int64_t o = (bh * 64 + d) * p.attn.tkp;
-      c.hi = (uint16_t*)p.attn.vh + o; c.lo = (uint16_t*)p.attn.vl + o; c.step = 1;
-    }
-  } else if (p.e_hi) {
+  if (p.e_hi) {
     const int64_t o = (int64_t)b * p.Lout * p.e_ld + n;
     c.hi = (uint16_t*)p.e_hi + o; c.lo = p.e_lo ? (uint16_t*)p.e_lo + o : nullptr; c.step = p.e_ld;
   }
   return c;
-}
-__device__ __forceinline__ void emit_store(const EmitCol& c, int64_t row, float v) {
-  uint16_t h, l;
-  if (c.f16) { __half a, b; split16(v * c.mul, a, b); h = __half_as_ushort(a); l = __half_as_ushort(b); }
-  else { __nv_bfloat16 a, b; split16(v, a, b); h = __bfloat16_as_ushort(a); l = __bfloat16_as_ushort(b); }
-  c.hi[row * c.step] = h;
-  if (c.lo) c.lo[row * c.step] = l;
 }
 
 // smem: [stages] x { A_hi 16 KB | A_lo 16 KB (planes==2) | W BN*128 B (x wplanes) }, then barriers.  After the K loop the stage
@@ -249,14 +229,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
       if (p.post_act) {
 #pragma unroll
         for (int i = 0; i < 32; i++) {
-          const float v = act_noinline(stage[i * LD + lane] + bias, p.post_act, p.post_p0) * cso + rr[i];
+          const float v = epilogue_value(stage[i * LD + lane], bias, p.post_act, p.post_p0, cso, rr[i]);
           yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
           if (ec.hi) emit_store(ec, row0 + i, v);
         }
       } else {
 #pragma unroll
         for (int i = 0; i < 32; i++) {
-          const float v = (stage[i * LD + lane] + bias) * cso + rr[i];
+          const float v = epilogue_value(stage[i * LD + lane], bias, 0, 0.f, cso, rr[i]);
           yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
           if (ec.hi) emit_store(ec, row0 + i, v);
         }

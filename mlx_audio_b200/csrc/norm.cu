@@ -4,6 +4,7 @@
 // applied for free inside the consuming conv's prologue (conv.cu: Pre).
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "layernorm_row.cuh"
 
 namespace {
 
@@ -133,62 +134,9 @@ __global__ void __launch_bounds__(128) layernorm_vec_kernel(const float* __restr
   pdl_wait();                                              // x / res are the preceding kernel's output
   const int64_t row = (int64_t)blockIdx.x * 4 + threadIdx.x / 32;
   if (row >= rows) return;
-  const int lane = threadIdx.x & 31;
-  const float4* xp = reinterpret_cast<const float4*>(x + row * x_ld);
-  const float4* rp = res ? reinterpret_cast<const float4*>(res + row * res_ld) : nullptr;
-  const int nv = C >> 2;
-  float4 v[NV];
-#pragma unroll
-  for (int j = 0; j < NV; j++) {
-    const int i = lane + 32 * j;
-    v[j] = i < nv ? xp[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (rp) {
-#pragma unroll
-    for (int j = 0; j < NV; j++) {
-      const int i = lane + 32 * j;
-      if (i < nv) { const float4 r = rp[i]; v[j].x += r.x; v[j].y += r.y; v[j].z += r.z; v[j].w += r.w; }
-    }
-  }
-  float s1 = 0.f;
-#pragma unroll
-  for (int j = 0; j < NV; j++) s1 += (v[j].x + v[j].y) + (v[j].z + v[j].w);
-  s1 = warp_sum(s1);
-  const float mean = rms ? 0.f : s1 / C;
-  float s2 = 0.f;
-#pragma unroll
-  for (int j = 0; j < NV; j++) {
-    if (lane + 32 * j < nv) {
-      const float a = v[j].x - mean, b = v[j].y - mean, c = v[j].z - mean, d = v[j].w - mean;
-      s2 = fmaf(a, a, s2); s2 = fmaf(b, b, s2); s2 = fmaf(c, c, s2); s2 = fmaf(d, d, s2);
-    }
-  }
-  s2 = warp_sum(s2);
-  const float rstd = rsqrtf(s2 / C + eps);
   pdl_launch_dependents();
-  float4* yp = reinterpret_cast<float4*>(y + row * y_ld);
-#pragma unroll
-  for (int j = 0; j < NV; j++) {
-    const int i = lane + 32 * j;
-    if (i < nv) {
-      float o[4] = {(v[j].x - mean) * rstd, (v[j].y - mean) * rstd, (v[j].z - mean) * rstd, (v[j].w - mean) * rstd};
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const int c = 4 * i + q;
-        if (ada) o[q] = fmaf(1.f + ada[c], o[q], ada[C + c]);
-        else { if (w) o[q] *= w[c]; if (bb) o[q] += bb[c]; }
-        if (post_act) o[q] = b2a_act(o[q], post_act, post_p0, 1.f, 1.f);
-      }
-      yp[i] = make_float4(o[0], o[1], o[2], o[3]);
-      if (e_hi) {
-        __align__(8) __nv_bfloat16 h[4], l[4];
-#pragma unroll
-        for (int q = 0; q < 4; q++) tc::split16(o[q], h[q], l[q]);
-        *reinterpret_cast<uint2*>(e_hi + row * e_ld + 4 * i) = *reinterpret_cast<const uint2*>(h);
-        if (e_lo) *reinterpret_cast<uint2*>(e_lo + row * e_ld + 4 * i) = *reinterpret_cast<const uint2*>(l);
-      }
-    }
-  }
+  layernorm_row_vec<NV>(x + row * x_ld, res ? res + row * res_ld : nullptr, y + row * y_ld, C, w, bb, ada, eps, rms, post_act, post_p0,
+                        e_hi ? e_hi + row * e_ld : nullptr, e_lo ? e_lo + row * e_ld : nullptr, threadIdx.x & 31);
 }
 
 }  // namespace

@@ -867,6 +867,49 @@ def attention(q, k, v, *, n_heads, n_kv_heads=None, scale, causal=False, q_offse
     return out
 
 
+_ALBERT_ERR = {}
+
+
+def albert_error_word(device) -> torch.Tensor:
+    """int32 [1] on ``device``: set to 1 by ``albert_encoder`` when one of its grid barriers saw no progress for 10 s (that call's
+    output is then invalid).  Never cleared."""
+    device = torch.device(device)
+    w = _ALBERT_ERR.get(device)
+    if w is None:
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("albert_encoder: run it once outside graph capture first (its error word is allocated then)")
+        w = _ALBERT_ERR[device] = torch.zeros(1, device=device, dtype=torch.int32)
+    return w
+
+
+def albert_encoder(h: torch.Tensor, hp: Planes, layers: int, qkv: ConvW, attn_out: ConvW, ffn: ConvW, ffn_out: ConvW, ln_attn, ln_full,
+                   *, heads: int, scale: float, eps: float, timeline: Optional[torch.Tensor] = None) -> None:
+    """``layers`` ALBERT layers on h [1, T, hidden] float32 and its bf16 planes ``hp``, both updated in place, in one persistent launch
+    (b2a_albert_encoder); bit-identical to the ``linear(qkv_heads=)`` / ``attention_planes`` / ``linear`` / ``layernorm(planes=True)``
+    sequence.  ``ln_attn`` / ``ln_full`` are (weight, bias) pairs; ``timeline`` int64 [layers * 7, SMs, 2] selects the profiling build."""
+    if h.dtype != torch.float32 or not h.is_contiguous() or h.dim() != 3 or h.shape[0] != 1:
+        raise ValueError(f"albert_encoder: h must be a contiguous float32 [1, T, hidden] tensor, got {tuple(h.shape)} {h.dtype}")
+    T, hs = h.shape[1], h.shape[2]
+    inter = ffn.cout
+    for cw, (n, k) in ((qkv, (3 * hs, hs)), (attn_out, (hs, hs)), (ffn, (inter, hs)), (ffn_out, (hs, inter))):
+        if cw.w_tc is None or cw.K != 1 or cw.f16 or cw.w_tc_lo is not None or (cw.cout, cw.cin_pad) != (n, k) or cw.bias is None:
+            raise ValueError("albert_encoder: every projection needs bf16 tensor-core weights with a bias and matching shapes")
+    two = TC_MODE[0] == "x2"
+    if hp.hi.shape != (1, T, hs) or (hp.lo is not None) != two:
+        raise ValueError("albert_encoder: hp must hold h's bf16 planes (hi, and lo in x2 mode)")
+    a = _lib.AlbertParams()
+    a.T, a.layers, a.heads, a.hidden, a.inter, a.planes = T, layers, heads, hs, inter, 2 if two else 1
+    for i, cw in enumerate((qkv, attn_out, ffn, ffn_out)):
+        a.w[i], a.bias[i] = cw.w_tc.data_ptr(), cw.bias.data_ptr()
+    a.ln_w[0], a.ln_b[0] = ln_attn[0].data_ptr(), ln_attn[1].data_ptr()
+    a.ln_w[1], a.ln_b[1] = ln_full[0].data_ptr(), ln_full[1].data_ptr()
+    a.eps, a.scale = eps, scale
+    a.h, a.h_hi, a.h_lo = h.data_ptr(), hp.hi.data_ptr(), _p(hp.lo)
+    err = albert_error_word(h.device)
+    ws = torch.empty(_lib.lib().b2a_albert_ws_bytes(T, heads, hs, inter), device=h.device, dtype=torch.uint8)
+    _call("albert", _lib.lib().b2a_albert_encoder, 1, C.byref(a), ws.data_ptr(), err.data_ptr(), _p(timeline), _stream())
+
+
 def attention_planes(ap: AttnPlanes, *, planes=False, out=None):
     """Non-causal tensor-core attention over the operands a fused qkv projection emitted (``linear(..., qkv_heads=)``): one launch.
     Returns ctx [B, T, H*64], or (ctx, Planes) with ``planes=True`` (ctx's bf16 planes for the output projection)."""

@@ -18,6 +18,7 @@ from __future__ import annotations
 import functools
 import math
 import time
+import weakref
 from dataclasses import dataclass
 from numbers import Number
 from typing import Dict, Optional
@@ -549,28 +550,17 @@ class Model:
                 te = ops.layernorm(te, lw, lb, eps=1e-5, post_act=ACT["lrelu"], post_p0=0.2)
             self._lstm_run(te[0], W["te_lstm"], out=t_en)
 
-        if par:
-            side_text = ops.fork(dev, 1)
-            with torch.cuda.stream(side_text[0]):
-                text_branch()
         # ---- ALBERT
         e = ops.gather_rows(W["word_emb"], ids)
         nh = cfg.plbert["num_attention_heads"]
         hs = cfg.plbert["hidden_size"]
         scale = 1.0 / math.sqrt(hs // nh)
         if self._albert_planes(T):
-            # 7 launches per layer: every producer also writes its consumer's 16-bit operand planes (no prep kernels), the qkv
-            # projection those of the attention; bit-identical to the branch below
+            # every layer in one persistent launch (csrc/albert.cu); bit-identical to the branch below
             _, ep = ops.layernorm(e, *W["emb_ln"], eps=1e-12, res=W["pos_type"][:T], planes=True)
             h, hp = ops.linear(ep, W["map_in"], planes=True)
-            for _ in range(cfg.plbert["num_hidden_layers"]):
-                _, qkv = ops.linear(hp, W["qkv"], qkv_heads=nh, qkv_scale=scale)
-                _, cp = ops.attention_planes(qkv, planes=True)
-                a = ops.linear(cp, W["attn_out"], res=h)
-                a, ap = ops.layernorm(a, *W["attn_ln"], eps=1e-12, planes=True)
-                _, fp = ops.linear(ap, W["ffn"], post_act=ACT["gelu"], planes=True)
-                f2 = ops.linear(fp, W["ffn_out"], res=a)
-                h, hp = ops.layernorm(f2, *W["full_ln"], eps=1e-12, planes=True)
+            ops.albert_encoder(h, hp, cfg.plbert["num_hidden_layers"], W["qkv"], W["attn_out"], W["ffn"], W["ffn_out"], W["attn_ln"],
+                               W["full_ln"], heads=nh, scale=scale, eps=1e-12)
             h = h[0]
         else:
             # The GEMMs stay on conv_tc like the chain's: above 256 rows the fused kernel would take them and split K across CTAs,
@@ -587,6 +577,10 @@ class Model:
                     f2 = ops.linear(f1, W["ffn_out"], res=a)
                     h = ops.layernorm(f2, *W["full_ln"], eps=1e-12)
         self._tap("bert", h)
+        if par:
+            side_text = ops.fork(dev, 1)
+            with torch.cuda.stream(side_text[0]):
+                text_branch()
         # ---- duration encoder: X640 = [d_en | style]
         stl = cfg.style_dim
         X = torch.empty(T, hd + stl, device=dev, dtype=torch.float32)
@@ -614,12 +608,13 @@ class Model:
         return st
 
     def _albert_planes(self, T: int) -> bool:
-        """ALBERT runs as the plane-emitting launch chain when every GEMM takes the tensor-core path at T rows and the attention the
-        tensor-core kernel (64-wide heads, at least 64 keys); otherwise (short utterances, B2A_TC=off, B2A_ATTN=cuda) as separate ops."""
+        """ALBERT runs as one persistent kernel (ops.albert_encoder) when every GEMM takes the tensor-core path at T rows and the
+        attention the tensor-core kernel (64-wide heads, 64 to 512 keys); otherwise (short or long utterances, B2A_TC=off,
+        B2A_ATTN=cuda) as separate ops."""
         W, pb = self._w, self.config.plbert
-        return (T >= 64 and ops.ATTN_MODE[0] == "tc" and pb["hidden_size"] == 64 * pb["num_attention_heads"]
+        return (64 <= T <= 512 and ops.ATTN_MODE[0] == "tc" and pb["hidden_size"] == 64 * pb["num_attention_heads"]
                 and pb["hidden_size"] % 64 == 0 and W["map_in"].cin % 64 == 0
-                and all(ops.emit_tc_eligible(W[k], T) for k in ("map_in", "qkv", "attn_out", "ffn", "ffn_out")))
+                and all(ops.emit_tc_eligible(W[k], T) and W[k].w_tc_lo is None for k in ("map_in", "qkv", "attn_out", "ffn", "ffn_out")))
 
     def _bind(self, st):
         """Point the style-projection lookups (`_gb`) at this utterance's rows."""
@@ -895,7 +890,9 @@ class Model:
     def _get_pipeline(self, lang_code: str, **kw):
         from .pipeline import KokoroPipeline
         if lang_code not in self._pipelines:
-            self._pipelines[lang_code] = KokoroPipeline(lang_code, self, self.repo_id, **kw)
+            # the cached pipeline refers back to the model weakly: a model <-> pipeline cycle would keep the model's weights and graphs
+            # in GPU memory after its last user reference is gone, until some later garbage-collection pass frees them
+            self._pipelines[lang_code] = KokoroPipeline(lang_code, weakref.proxy(self), self.repo_id, **kw)
         return self._pipelines[lang_code]
 
     def _result(self, audio, seg_idx, n_tokens, seg_t):

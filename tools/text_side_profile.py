@@ -4,7 +4,8 @@ Builds the cfg2 model as bench.py does (synthetic checkpoint, 128 phonemes -> T 
 external event node around every launch, replays it and prints, per stage, the launches per ALBERT layer and their in-graph time, then
 the text-graph replay time and its launch count.  Stages are read off the line of `Model._text_side` that issued each launch, so the
 script attributes any version of that function.  The sum of in-graph times over-counts wall time where the text-encoder branch runs
-concurrently on its side stream; the replay time is the wall time.
+concurrently on its side stream; the replay time is the wall time.  When ALBERT runs as the persistent kernel, eager calls of its
+timeline build then give each stage's time per layer and the barrier wait in front of it.
 
     python tools/text_side_profile.py [--reps 20] [--json OUT]
 """
@@ -21,12 +22,42 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 # (stage, substring of the issuing source line); first match wins
-STAGES = [("attention", "attention"), ("qkv", 'W["qkv"]'), ("attn_out", 'W["attn_out"]'), ("attn_ln", 'W["attn_ln"]'),
+STAGES = [("ALBERT (persistent)", "albert_encoder"), ("attention", "attention"), ("qkv", 'W["qkv"]'), ("attn_out", 'W["attn_out"]'), ("attn_ln", 'W["attn_ln"]'),
           ("ffn_out", 'W["ffn_out"]'), ("ffn", 'W["ffn"]'), ("full_ln", 'W["full_ln"]'),
           ("embedding", 'W["emb_ln"]'), ("embedding", 'W["map_in"]'), ("embedding", 'W["word_emb"]'),
           ("text encoder branch", "text_branch"), ("bert_encoder", 'W["bert_encoder"]'), ("duration LSTMs + AdaLN", "dur_lstms"),
           ("duration LSTMs + AdaLN", "adaln"), ("duration head", "pred_lstm"), ("duration head", 'W["dur_')]
-ALBERT = ["qkv", "attention", "attn_out", "attn_ln", "ffn", "ffn_out", "full_ln"]
+ALBERT = ["ALBERT (persistent)", "qkv", "attention", "attn_out", "attn_ln", "ffn", "ffn_out", "full_ln"]
+KERNEL_STAGES = ["qkv", "attention", "attn_out", "attn_ln", "ffn", "ffn_out", "full_ln"]      # csrc/albert.cu, per layer
+
+
+def albert_timeline(model, ids, ref_s, layers, reps):
+    """Per-stage times of the persistent kernel from its timeline build: globaltimer at the start (after the grid barrier) and end of
+    every stage of every CTA.  Returns {stage: (us from the first CTA's start to the last CTA's end, mean us a CTA waits at the
+    barrier in front of it)} averaged over layers and eager calls."""
+    import torch
+    from mlx_audio_b200 import ops
+    nsm = torch.cuda.get_device_properties(model.device).multi_processor_count
+    tl = torch.zeros(layers * 7, nsm, 2, dtype=torch.int64, device=model.device)
+    orig = ops.albert_encoder
+    span = [0.0] * 7
+    wait = [0.0] * 7
+    ops.albert_encoder = lambda *a, **k: orig(*a, **k, timeline=tl)
+    try:
+        for _ in range(reps + 1):
+            model._text_side(ids, ref_s)
+            torch.cuda.synchronize()
+            t = tl.double().cpu()
+            if _ == 0:
+                continue                                               # warm-up
+            for k in range(layers * 7):
+                span[k % 7] += float(t[k, :, 1].max() - t[k, :, 0].min()) / 1e3
+                if k:
+                    wait[k % 7] += float((t[k, :, 0] - t[k - 1, :, 1]).mean()) / 1e3
+    finally:
+        ops.albert_encoder = orig
+    n = reps * layers
+    return {st: (span[i] / n, wait[i] / n) for i, st in enumerate(KERNEL_STAGES)}
 
 
 def _stage() -> str:
@@ -136,11 +167,21 @@ def main() -> None:
     n_kernels = sum(n for _, _, n, _, _ in rec)
     print(f"ALBERT layers: {albert_k / layers:.0f} kernels and {albert_us / layers:.1f} us per layer, {albert_us:.1f} us in all")
     print(f"text graph: {n_kernels} kernels, replay {replay_ms:.3f} ms")
+    timeline = None
+    if "ALBERT (persistent)" in stages:
+        timeline = albert_timeline(model, ids[0].to(dev), ref_s.to(dev), layers, args.reps)
+        print("persistent ALBERT kernel, timeline build (eager calls), per layer:")
+        print(f"{'stage':<12}{'us':>8}{'barrier wait us':>17}")
+        for st, (us, w) in timeline.items():
+            print(f"{st:<12}{us:>8.1f}{w:>17.1f}")
+        print(f"{'sum':<12}{sum(v[0] for v in timeline.values()):>8.1f}{sum(v[1] for v in timeline.values()):>17.1f}")
     res = {"device": name, "T": T, "reps": args.reps, "text_graph_ms": round(replay_ms, 4), "text_graph_kernels": n_kernels,
            "albert_kernels_per_layer": albert_k / layers, "albert_us_per_layer": round(albert_us / layers, 2),
            "stages": {k: {"kernels": v["kernels"], "us": round(v["us"], 1),
                           "entry_points": {e: {"kernels": x["kernels"], "us": round(x["us"], 1)} for e, x in v["entry_points"].items()}}
-                      for k, v in stages.items()}}
+                      for k, v in stages.items()},
+           "albert_timeline_us": None if timeline is None else {k: {"us": round(v[0], 2), "barrier_wait_us": round(v[1], 2)}
+                                                               for k, v in timeline.items()}}
     print(json.dumps(res))
     if args.json:
         with open(args.json, "w") as f:
