@@ -231,7 +231,8 @@ int32_t b2a_rope(float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T, int
 /* ---- bidirectional LSTM recurrence (modules.py:93-285) ------------------------------------
  * xproj [B,T,2,4H] = x @ Wx^T + b_ih + b_hh for (forward|backward), gate order i,f,g,o;
  * wh [2,4H,H]; out [B,T,2H] (forward | backward).  H must be 256 (Kokoro) -- one 8-CTA cluster
- * per (direction, batch) keeps Wh in registers and exchanges h through distributed shared memory. */
+ * per (direction, batch) keeps Wh in registers; each warp runs its 4 hidden units' step on its own and
+ * pushes their new h into every CTA's shared memory (distributed shared memory, one mbarrier per step). */
 int32_t b2a_lstm_bidir(const float* xproj, const float* wh, float* out, int64_t out_ld, int32_t B, int32_t T, int32_t H, void* stream);
 
 /* ---- DSP ------------------------------------------------------------------------------------
