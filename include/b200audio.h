@@ -434,6 +434,35 @@ int32_t b2a_snac_from_codes(const int64_t* const* codes_host_ptrs, const int32_t
                             const float* const* emb_host_ptrs, const float* const* w_host_ptrs, const float* const* bias_host_ptrs,
                             int32_t B, int64_t T, int32_t bins, int32_t cd, int32_t dim, float* out, int32_t* err_flag_dev, void* stream);
 
+/* ---- Descript Audio Codec quantiser (dac.cu; codec/models/descript/nn/quantize.py) ------------------------------------------
+ * One level of the factorised residual quantiser, all pointers to DEVICE memory; the table of levels itself lives in device memory.
+ * w_in [dim][cd] and w_out [cd][dim] are the weight-norm-folded 1x1 projections in packed (K = 1) conv layout, cb the code book
+ * [bins][cd], cbn its rows L2-normalised (x / max(|x|, 1e-12), rounded to fp32), c2[i] = |cbn[i]|^2 in float64.  lat_off = the level's
+ * first channel in the concatenated latents (sum of the previous levels' cd).  Decode reads cb, w_out, b_out, cd, lat_off only. */
+typedef struct {
+  const float* w_in; const float* b_in;
+  const float* cbn; const double* c2;
+  const float* cb;
+  const float* w_out; const float* b_out;
+  int32_t cd; int32_t lat_off;
+} b2a_dac_level_t;
+/* ResidualVectorQuantize.__call__ (quantize.py:87-120 over VectorQuantize.__call__ / decode_latents :25-63) in one launch, for
+ * n_levels <= the model's code books: per level z_e = w_in r + b_in, idx = argmin_i |z_e/|z_e||^2 - 2 z_e/|z_e| . cbn_i + |cbn_i|^2 (float64
+ * scores, lowest index on ties), z_q_l = w_out cb[idx] + b_out, r -= z_q_l.  z [B*T, dim] fp32 rows (row stride z_ld, channels-last);
+ * outputs codes int64 [B, n_levels, T], latents [B, latent_channels, T] (the un-normalised z_e of every level), z_q [B, T, dim] and
+ * loss_part float64 [ceil(B*T / 8)]: its sum is the reference's commitment loss (= its codebook loss in the forward pass), the per-level
+ * mean of (z_e - cb[idx])^2 summed over levels.  z == NULL runs from_latents (quantize.py:133-151) instead: z_e is READ from latents.
+ * A CTA holds 8 frames' residual and z_q in b2a_dac_rvq_encode_smem_bytes of dynamic shared memory. */
+int64_t b2a_dac_rvq_encode_smem_bytes(int32_t dim);
+int32_t b2a_dac_rvq_encode(const float* z, int64_t z_ld, int32_t B, int64_t T, int32_t dim, const b2a_dac_level_t* levels_dev, int32_t n_levels,
+                           int32_t bins, int32_t latent_channels, int64_t* codes, float* latents, float* z_q, double* loss_part, void* stream);
+/* ResidualVectorQuantize.from_codes (quantize.py:122-131) for the first n_levels code books: out[b,t,:] = sum_l ( w_out_l cb_l[codes[b,l,t]]
+ * + b_out_l ), and z_p [B, latent_channels, T] = the gathered rows (NULL: not wanted).  codes int64, element (b, l, t) at b * codes_bs +
+ * l * codes_qs + t.  A code outside [0, bins) sets *err_flag_dev (and decodes as 0). */
+int32_t b2a_dac_from_codes(const int64_t* codes, int64_t codes_bs, int64_t codes_qs, int32_t B, int32_t n_levels, int64_t T,
+                           const b2a_dac_level_t* levels_dev, int32_t bins, int32_t latent_channels, int32_t dim, float* out, float* z_p,
+                           int32_t* err_flag_dev, void* stream);
+
 /* ---- streaming decoder state (stream.cu) ------------------------------------------------------
  * One entry of a grouped row-range launch on fp32 [B, rows, C] views: dst[b, r, c] = src[b, r, c] (COPY) or += (ADD), element
  * (b, r, c) at b * bs + r * ld + c.  The incremental Qwen3-TTS speech-tokenizer decoder keeps its state with it:

@@ -74,6 +74,12 @@ class RowOp(C.Structure):
                 ("B", i32), ("rows", i32), ("C", i32), ("op", i32)]
 
 
+class DacLevel(C.Structure):
+    """Mirror of b2a_dac_level_t."""
+    _fields_ = [("w_in", C.c_void_p), ("b_in", C.c_void_p), ("cbn", C.c_void_p), ("c2", C.c_void_p), ("cb", C.c_void_p),
+                ("w_out", C.c_void_p), ("b_out", C.c_void_p), ("cd", i32), ("lat_off", i32)]
+
+
 ROWOPS_MAX = 32      # B2A_ROWOPS_MAX
 
 
@@ -136,6 +142,9 @@ PROTOTYPES = {
     "b2a_rvq_encode": (i32, [c_f, i64, i64, i32, c_f, c_f, i32, i32, i32, c_f, i64, i64, C.c_void_p]),
     "b2a_snac_from_codes": (i32, [C.POINTER(C.c_void_p), C.POINTER(i32), i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                   C.POINTER(C.c_void_p), i32, i64, i32, i32, i32, c_f, c_f, C.c_void_p]),
+    "b2a_dac_rvq_encode_smem_bytes": (i64, [i32]),
+    "b2a_dac_rvq_encode": (i32, [c_f, i64, i32, i64, i32, c_f, i32, i32, i32, c_f, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_dac_from_codes": (i32, [c_f, i64, i64, i32, i32, i64, c_f, i32, i32, i32, c_f, c_f, c_f, C.c_void_p]),
     "b2a_stream_rows": (i32, [C.POINTER(RowOp), i32, C.c_void_p]),
     "b2a_conv1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, i32, c_f, i32, C.c_void_p]),
     "b2a_convtr1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, C.c_void_p]),

@@ -1,4 +1,5 @@
+from .models.dac import DAC, DACFile
 from .models.mimi import Mimi, MimiConfig, MimiStreamingDecoder, mimi_202407
 from .models.snac import SNAC
 
-__all__ = ["Mimi", "MimiConfig", "MimiStreamingDecoder", "mimi_202407", "SNAC"]
+__all__ = ["Mimi", "MimiConfig", "MimiStreamingDecoder", "mimi_202407", "SNAC", "DAC", "DACFile"]

@@ -1262,6 +1262,57 @@ def snac_from_codes(codes, strides, embs, ws, biases, dim: int, check=True) -> t
     return out
 
 
+def dac_levels(levels, device) -> torch.Tensor:
+    """Device-side table of b2a_dac_level_t from ``levels``: dicts of CUDA tensors {w_in, b_in, cbn, c2, cb, w_out, b_out} (w_in / b_in /
+    cbn / c2 None for a decode-only table).  The returned uint8 tensor keeps the table; the caller keeps the tensors it points to."""
+    arr = (_lib.DacLevel * len(levels))()
+    off = 0
+    for a, lv in zip(arr, levels):
+        for k in ("w_in", "b_in", "cbn", "c2", "cb", "w_out", "b_out"):
+            t = lv.get(k)
+            assert t is None or (t.is_cuda and t.is_contiguous() and t.dtype == (torch.float64 if k == "c2" else torch.float32))
+            setattr(a, k, _p(t))
+        a.cd, a.lat_off = lv["cb"].shape[1], off
+        off += a.cd
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(device)
+
+
+def dac_rvq_encode(z: Optional[torch.Tensor], table: torch.Tensor, n_levels: int, bins: int, lat_ch: int, dim: int, *,
+                   latents: Optional[torch.Tensor] = None):
+    """DAC residual quantiser, all ``n_levels`` in one launch: z [B, T, dim] fp32 -> (codes int64 [B, n_levels, T], latents [B, lat_ch, T],
+    z_q [B, T, dim], loss_part float64 [CTAs] whose sum is the commitment (= codebook) loss).  ``z=None`` with ``latents`` given runs
+    from_latents: the search and the out-projections on the given z_e, no residual."""
+    if z is not None:
+        _chk3(z, "dac_rvq_encode z")
+        assert z.is_contiguous() and z.shape[2] == dim
+        B, T, _ = z.shape
+        latents = torch.empty(B, lat_ch, T, device=z.device, dtype=torch.float32)
+    else:
+        assert latents.dtype == torch.float32 and latents.is_cuda and latents.is_contiguous() and latents.shape[1] == lat_ch
+        B, _, T = latents.shape
+    dev = latents.device
+    codes = torch.empty(B, n_levels, T, device=dev, dtype=torch.int64)
+    zq = torch.empty(B, T, dim, device=dev, dtype=torch.float32)
+    loss = torch.empty(-(-B * T // 8), device=dev, dtype=torch.float64)
+    _call("rvq", _lib.lib().b2a_dac_rvq_encode, 1, _p(z), dim, B, T, dim, table.data_ptr(), n_levels, bins, lat_ch, codes.data_ptr(),
+          latents.data_ptr(), zq.data_ptr(), loss.data_ptr(), _stream())
+    return codes, latents, zq, loss
+
+
+def dac_from_codes(codes: torch.Tensor, table: torch.Tensor, bins: int, lat_ch: int, dim: int, *, want_zp=False, check=True):
+    """DAC quantizer.from_codes for the first codes.shape[1] code books: codes int64 [B, nq, T] -> (z_q [B, T, dim], z_p [B, lat_ch, T] or None)."""
+    assert codes.dtype == torch.int64 and codes.is_cuda and codes.dim() == 3 and (codes.stride(2) == 1 or codes.shape[2] == 1)
+    B, nq, T = codes.shape
+    out = torch.empty(B, T, dim, device=codes.device, dtype=torch.float32)
+    zp = torch.empty(B, lat_ch, T, device=codes.device, dtype=torch.float32) if want_zp else None
+    err = torch.zeros(1, device=codes.device, dtype=torch.int32)
+    _call("rvq", _lib.lib().b2a_dac_from_codes, 1, codes.data_ptr(), codes.stride(0), codes.stride(1), B, nq, T, table.data_ptr(), bins, lat_ch,
+          dim, out.data_ptr(), _p(zp), err.data_ptr(), _stream())
+    if check and int(err.item()) != 0:
+        raise ValueError(f"dac_from_codes: code index out of range [0, {bins})")
+    return out, zp
+
+
 # ---------------------------------------------------------------------------------------------------------------- speaker encoder
 def spk_logmel(x: torch.Tensor, window: torch.Tensor, filters: torch.Tensor) -> torch.Tensor:
     """Qwen3-TTS speaker log-mel (qwen3_tts.py:64-121): x [B, n] float32 -> [B, frames, n_mels]; ``window`` [1024], ``filters`` [n_mels, 513]."""

@@ -256,6 +256,68 @@ def snac_noises(cfg, batch=1, seed=7):
     return [torch.randn(batch, 1, cfg["decoder_dim"] // (2 ** (i + 1)), generator=gen) for i in range(len(cfg["decoder_rates"]))]
 
 
+def dac_weights(cfg, seed=8, encoder=True):
+    """Parameter tree of codec/models/descript/dac.py:DAC (quantizer + decoder; ``encoder=True`` adds the encoder and the quantizers'
+    in_proj), random values by the recipe of ``snac_weights``: weight_v ~ N(0, 1/fan_in), weight_g = ||v|| rounded to bf16 (so the folded
+    weight is NOT 16-bit exact and the split-plane weight path runs), Snake alpha ~ U(0.5, 1.5) in the reference's [1, 1, C] layout.
+    Transposed convs are (out, K, in) with the norm per input channel (nn/layers.py:89-92)."""
+    g = _Gen(seed)
+    gen = g.g
+
+    def wn(pre, shape, fan_in, except_dim=0, bias=None):
+        v = _fan(g, pre + ".weight_v", *shape, fan_in=fan_in)
+        axes = tuple(i for i in range(3) if i != except_dim)
+        g.P[pre + ".weight_g"] = _bf16(torch.sqrt((v * v).sum(dim=axes, keepdim=True)))
+        if bias:
+            g.normal(pre + ".bias", bias, std=0.05)
+
+    def alpha(name, c):
+        g.P[name] = _bf16(0.5 + torch.rand(1, 1, c, generator=gen))
+
+    def res_units(bp, first, c):
+        for i in range(3):
+            rp = f"{bp}.{first + i}.block.layers"
+            alpha(rp + ".0.alpha", c)
+            wn(rp + ".1", (c, 7, c), 7 * c, bias=c)
+            alpha(rp + ".2.alpha", c)
+            wn(rp + ".3", (c, 1, c), c, bias=c)
+
+    latent = cfg.get("latent_dim") or cfg["encoder_dim"] * (2 ** len(cfg["encoder_rates"]))
+    cds = [cfg["codebook_dim"]] * cfg["n_codebooks"] if isinstance(cfg["codebook_dim"], int) else list(cfg["codebook_dim"])
+    for i, cd in enumerate(cds):
+        q = f"quantizer.quantizers.{i}"
+        g.normal(q + ".codebook.weight", cfg["codebook_size"], cd, std=1.0)
+        wn(q + ".out_proj", (latent, 1, cd), cd, bias=latent)
+    pre = "decoder.model.layers"
+    ch = cfg["decoder_dim"]
+    wn(f"{pre}.0", (ch, 7, latent), 7 * latent, bias=ch)
+    for i, stride in enumerate(cfg["decoder_rates"]):
+        cin, cout = ch // (2 ** i), ch // (2 ** (i + 1))
+        bp = f"{pre}.{i + 1}.block.layers"
+        alpha(f"{bp}.0.alpha", cin)
+        wn(f"{bp}.1", (cout, 2 * stride, cin), cin * 2, except_dim=2, bias=cout)         # ~2 taps hit each output
+        res_units(bp, 2, cout)
+    n = len(cfg["decoder_rates"])
+    alpha(f"{pre}.{n + 1}.alpha", cout)
+    wn(f"{pre}.{n + 2}", (1, 7, cout), 7 * cout * FINAL_GAIN_DIV, bias=1)
+    if encoder:                                                   # drawn AFTER the decode-side tensors: those keep their values
+        for i, cd in enumerate(cds):
+            wn(f"quantizer.quantizers.{i}.in_proj", (cd, 1, latent), latent, bias=cd)
+        pre = "encoder.block.layers"
+        d = cfg["encoder_dim"]
+        wn(f"{pre}.0", (d, 7, 1), 7, bias=d)
+        for i, stride in enumerate(cfg["encoder_rates"]):
+            bp = f"{pre}.{i + 1}.block.layers"
+            res_units(bp, 0, d)
+            alpha(f"{bp}.3.alpha", d)
+            wn(f"{bp}.4", (2 * d, 2 * stride, d), 2 * stride * d, bias=2 * d)
+            d *= 2
+        n = len(cfg["encoder_rates"])
+        alpha(f"{pre}.{n + 1}.alpha", d)
+        wn(f"{pre}.{n + 2}", (latent, 3, d), 3 * d, bias=latent)
+    return g.P
+
+
 def mimi_weights(cfg, seed=5, encoder=False):
     """Parameter tree of codec/models/mimi/mimi.py:Mimi (decode side; ``encoder=True`` adds the SEANet encoder, the encoder transformer, the
     down-sampling conv and the quantisers' input projections), random values at the mimi_202407 shapes."""
