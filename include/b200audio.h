@@ -463,6 +463,19 @@ int32_t b2a_dac_from_codes(const int64_t* codes, int64_t codes_bs, int64_t codes
                            const b2a_dac_level_t* levels_dev, int32_t bins, int32_t latent_channels, int32_t dim, float* out, float* z_p,
                            int32_t* err_flag_dev, void* stream);
 
+/* ---- BigVGAN anti-aliased activation (bigvgan.cu; codec/models/bigvgan/resample.py, activation.py) ---------------------------
+ * Activation1d(SnakeBeta) (resample.py:157-177, activation.py:42-51) in one pass: x [B, L, C] fp32 (element (b, t, c) at b * x_bs +
+ * t * x_ld + c) -> [B, L, C].  UpSample1d (resample.py:122-136): edge pad 5 rows, MLX conv_transpose1d scatter y[2i + k] += x[i] f_up[k]
+ * (no kernel flip) per channel, times 2, crop 15 rows each side; SnakeBeta v = u + inv_beta[c] sin(alpha[c] u)^2 with the Snake sine of
+ * common.cuh; alpha = exp(alpha) and inv_beta = 1 / (exp(beta) + 1e-9) precomputed per channel for snake_logscale; DownSample1d
+ * (resample.py:79-98): edge pad 5 | 6 rows of v, 12-tap f_down at stride 2.  f_up / f_down: the 12 taps as the checkpoint holds them.
+ * Output either fp32 y (row stride y_ld, batch stride y_bs) or the next tensor-core conv's bf16 planes hi / lo (lo may be NULL)
+ * [B, L, cpad] contiguous, pad channels zeroed, split as b2a_prep_bf16 splits them; exactly one of y / hi.  ratio 2 and 12 taps
+ * only (all BigVGAN uses): anything else is B2A_E_UNSUPPORTED.  Fixed tap order: bit-reproducible, independent of B. */
+int32_t b2a_aa_snakebeta(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t C, const float* alpha, const float* inv_beta,
+                         const float* f_up, const float* f_down, int32_t ratio, int32_t taps, float* y, int64_t y_bs, int64_t y_ld, void* hi,
+                         void* lo, int32_t cpad, void* stream);
+
 /* ---- streaming decoder state (stream.cu) ------------------------------------------------------
  * One entry of a grouped row-range launch on fp32 [B, rows, C] views: dst[b, r, c] = src[b, r, c] (COPY) or += (ADD), element
  * (b, r, c) at b * bs + r * ld + c.  The incremental Qwen3-TTS speech-tokenizer decoder keeps its state with it:

@@ -145,6 +145,7 @@ PROTOTYPES = {
     "b2a_dac_rvq_encode_smem_bytes": (i64, [i32]),
     "b2a_dac_rvq_encode": (i32, [c_f, i64, i32, i64, i32, c_f, i32, i32, i32, c_f, c_f, c_f, c_f, C.c_void_p]),
     "b2a_dac_from_codes": (i32, [c_f, i64, i64, i32, i32, i64, c_f, i32, i32, i32, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_aa_snakebeta": (i32, [c_f, i64, i64, i32, i32, i32, c_f, c_f, c_f, c_f, i32, i32, c_f, i64, i64, c_f, c_f, i32, C.c_void_p]),
     "b2a_stream_rows": (i32, [C.POINTER(RowOp), i32, C.c_void_p]),
     "b2a_conv1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, i32, c_f, i32, C.c_void_p]),
     "b2a_convtr1d_stream": (i32, [C.POINTER(Conv1dParams), c_f, i64, C.c_void_p]),

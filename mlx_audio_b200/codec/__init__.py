@@ -1,5 +1,6 @@
+from .models.bigvgan import BigVGAN, BigVGANConfig
 from .models.dac import DAC, DACFile
 from .models.mimi import Mimi, MimiConfig, MimiStreamingDecoder, mimi_202407
 from .models.snac import SNAC
 
-__all__ = ["Mimi", "MimiConfig", "MimiStreamingDecoder", "mimi_202407", "SNAC", "DAC", "DACFile"]
+__all__ = ["Mimi", "MimiConfig", "MimiStreamingDecoder", "mimi_202407", "SNAC", "DAC", "DACFile", "BigVGAN", "BigVGANConfig"]

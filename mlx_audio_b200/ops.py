@@ -1313,6 +1313,34 @@ def dac_from_codes(codes: torch.Tensor, table: torch.Tensor, bins: int, lat_ch: 
     return out, zp
 
 
+# ---------------------------------------------------------------------------------------------------------------- BigVGAN
+def aa_snakebeta(x: torch.Tensor, a: torch.Tensor, inv_b: torch.Tensor, f_up: torch.Tensor, f_down: torch.Tensor, *,
+                 planes_for: Optional[ConvW] = None):
+    """BigVGAN's Activation1d(SnakeBeta) (resample.py:157-177) in one launch: x [B, L, C] -> fp32 [B, L, C], or with ``planes_for`` the
+    bf16 ``Planes`` [B, L, planes_for.cin_pad] that ``conv1d(planes, planes_for, ...)`` takes with no prologue.  ``a`` / ``inv_b`` [C]:
+    the SnakeBeta gains as the kernel applies them (exp(alpha), 1 / (exp(beta) + 1e-9) for snake_logscale); ``f_up`` / ``f_down``: the
+    12 taps of the up- and down-sampling filters."""
+    _chk3(x, "aa_snakebeta x")
+    B, L, Cc = x.shape
+    for name, t, n in (("a", a, Cc), ("inv_b", inv_b, Cc), ("f_up", f_up, f_up.numel()), ("f_down", f_down, f_down.numel())):
+        if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or t.numel() != n:
+            raise ValueError(f"aa_snakebeta: {name} must be a contiguous CUDA float32 tensor of {n} values")
+    if f_up.numel() != f_down.numel():
+        raise ValueError("aa_snakebeta: the up- and down-sampling filters must have the same number of taps")
+    if planes_for is not None:
+        if planes_for.cin != Cc or planes_for.w_tc is None or planes_for.f16:
+            raise ValueError("aa_snakebeta: planes_for must be a bf16 tensor-core conv taking the activation's channels")
+        out = _new_planes(B, L, planes_for.cin_pad, x.device)
+        out.C = Cc
+        _call("aa_act", _lib.lib().b2a_aa_snakebeta, 1, x.data_ptr(), x.stride(0), x.stride(1), B, L, Cc, a.data_ptr(), inv_b.data_ptr(),
+              f_up.data_ptr(), f_down.data_ptr(), 2, f_up.numel(), None, 0, 0, out.hi.data_ptr(), _p(out.lo), planes_for.cin_pad, _stream())
+        return out
+    out = torch.empty(B, L, Cc, device=x.device, dtype=torch.float32)
+    _call("aa_act", _lib.lib().b2a_aa_snakebeta, 1, x.data_ptr(), x.stride(0), x.stride(1), B, L, Cc, a.data_ptr(), inv_b.data_ptr(),
+          f_up.data_ptr(), f_down.data_ptr(), 2, f_up.numel(), out.data_ptr(), out.stride(0), out.stride(1), None, None, 0, _stream())
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------------------- speaker encoder
 def spk_logmel(x: torch.Tensor, window: torch.Tensor, filters: torch.Tensor) -> torch.Tensor:
     """Qwen3-TTS speaker log-mel (qwen3_tts.py:64-121): x [B, n] float32 -> [B, frames, n_mels]; ``window`` [1024], ``filters`` [n_mels, 513]."""

@@ -318,6 +318,37 @@ def dac_weights(cfg, seed=8, encoder=True):
     return g.P
 
 
+BIGVGAN_FINAL_GAIN = 0.01  # conv_post's gain: keeps the pre-tanh signal of the deep unit-gain stack mostly inside the unsaturated range
+
+
+def bigvgan_weights(cfg, seed=9):
+    """Parameter tree of codec/models/bigvgan/bigvgan.py:BigVGAN (``cfg`` a BigVGANConfig), without the resampling filters (the model
+    computes them, as the reference's constructor does).  Unit-gain convs by the recipe of ``dac_weights`` (weight_v ~ N(0, 1/fan_in),
+    weight_g = ||v|| rounded to bf16), transposed convs (out, K, in) with the norm per input channel (conv.py:91); SnakeBeta alpha / beta
+    ~ 0.1 N(0, 1) for snake_logscale (exp ~ 1) and U(0.5, 1.5) otherwise; conv_post scaled by BIGVGAN_FINAL_GAIN."""
+    from .codec.models.bigvgan import param_shapes
+    g = _Gen(seed)
+    for name, shape in param_shapes(cfg).items():
+        leaf = name.rsplit(".", 1)[-1]
+        if leaf == "filter" or leaf == "weight_g":
+            continue
+        if leaf == "weight_v":
+            pre = name[: -len(".weight_v")]
+            tr = pre.startswith("ups.")
+            cout, k, cin = shape
+            fan_in = cin * 2 if tr else cin * k                      # a transposed conv with K = 2 u hits each output with ~2 taps
+            v = _fan(g, name, *shape, fan_in=fan_in)
+            norm = torch.sqrt((v * v).sum(dim=(0, 1) if tr else (1, 2), keepdim=True))
+            g.P[pre + ".weight_g"] = _bf16(norm * (BIGVGAN_FINAL_GAIN if pre == "conv_post" else 1.0))
+        elif leaf == "bias":
+            g.normal(name, *shape, std=0.05)
+        elif cfg.snake_logscale:
+            g.normal(name, *shape, std=0.1)
+        else:
+            g.P[name] = _bf16(0.5 + torch.rand(*shape, generator=g.g))
+    return g.P
+
+
 def mimi_weights(cfg, seed=5, encoder=False):
     """Parameter tree of codec/models/mimi/mimi.py:Mimi (decode side; ``encoder=True`` adds the SEANet encoder, the encoder transformer, the
     down-sampling conv and the quantisers' input projections), random values at the mimi_202407 shapes."""
