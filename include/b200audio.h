@@ -570,6 +570,31 @@ int32_t b2a_spk_asp_act(float* h, int64_t h_bs, int64_t h_ld, const float* cb, i
 int32_t b2a_spk_asp_pool(const float* logits, int64_t l_bs, int64_t l_ld, const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T,
                          int32_t C, float eps, float* pooled, int64_t p_bs, void* stream);
 
+/* ---- Vocos (vocos.cu; codec/models/vocos/vocos.py, mel.py, dsp.py:385-513) ---------------------------------------------------
+ * ConvNeXtBlock's dwconv + norm (vocos.py:183-187), or with K == 0 VocosBackbone's norm / final_layer_norm (:263-274), in one pass:
+ * x [B, L, C] fp32 (element (b, t, c) at b * x_bs + t * x_ld + c).  dw_w [K, C] + dw_b [C] (or NULL): a depthwise conv with zero "same"
+ * padding K / 2, taps summed in ascending order; K odd <= 15, or 0 for no conv.  LayerNorm over C (eps from the caller, fp32 statistics
+ * in a fixed order), then either w (or NULL) and b (or NULL: final_layer_norm with bias=False), or, when ada != NULL, AdaLayerNorm's
+ * per-row scale v + shift (vocos.py:209-214) from ada[b * ada_bs + c] (scale) and ada[b * ada_bs + C + c] (shift).  Output fp32 y (row
+ * stride y_ld, batch stride y_bs; may be NULL), and / or the next GEMM's bf16 planes hi / lo (lo may be NULL) [B, L, C] contiguous,
+ * C % 64 == 0.  C % 4 == 0, C <= 1024, 16-byte aligned rows.  A batch row's result does not depend on B. */
+int32_t b2a_vocos_dwnorm(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t C, const float* dw_w, const float* dw_b,
+                         int32_t K, const float* w, const float* b, const float* ada, int64_t ada_bs, float eps, float* y, int64_t y_bs,
+                         int64_t y_ld, void* hi, void* lo, void* stream);
+/* ISTFTHead after its linear (vocos.py:126-140 with dsp.py:436-513): h [B, T, h_ld], h_ld >= n_fft + 2 (the linear's padded row), holds
+ * log-magnitudes in columns [0, n_fft/2 + 1) and phases in the next n_fft/2 + 1.  S = min(exp(mag), 100) (cos p + i sin p); irfft per
+ * frame (imaginary parts of the DC and Nyquist bins ignored), times the symmetric Hann `window` [n_fft], overlap-add at `hop`, divided by
+ * the summed window where that sum is > 1e-10, n_fft / 2 trimmed at each end: out [B, (T - 1) hop] (batch stride out_bs).  Gathered per
+ * output sample -- no workspace, no scatter; frames and bins summed in ascending order.  Even n_fft <= 2048 (1280 included), else
+ * B2A_E_UNSUPPORTED. */
+int32_t b2a_vocos_istft_head(const float* h, int64_t h_bs, int64_t h_ld, int32_t B, int32_t T, int32_t n_fft, int32_t hop, const float* window,
+                             float* out, int64_t out_bs, void* stream);
+/* mel.py:8-33 (log_mel_spectrogram) at n_fft 1024 / hop 256 on b2a_spk_logmel's kernel: reflect pad n_fft / 2 = 512 (no repeated edge),
+ * symmetric Hann `window` [1024], |X| (no epsilon) @ filters^T (HTK, norm None, [n_mels, 513]), log(max(., 1e-5)); the stft's last frame
+ * is dropped and never computed.  x [B, n] (row stride x_bs), n > 512; out [B, frames, n_mels] contiguous with frames = n / 256. */
+int32_t b2a_vocos_logmel(const float* x, int64_t x_bs, int32_t B, int64_t n, const float* window, const float* filters, int32_t n_mels,
+                         int64_t frames, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

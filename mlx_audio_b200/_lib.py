@@ -162,6 +162,9 @@ PROTOTYPES = {
     "b2a_spk_gemv": (i32, [c_f, i64, i32, i32, c_f, i64, i32, c_f, i32, c_f, i64, C.c_void_p]),
     "b2a_spk_asp_act": (i32, [c_f, i64, i64, c_f, i32, i32, i32, C.c_void_p]),
     "b2a_spk_asp_pool": (i32, [c_f, i64, i64, c_f, i64, i64, i32, i32, i32, f32, c_f, i64, C.c_void_p]),
+    "b2a_vocos_dwnorm": (i32, [c_f, i64, i64, i32, i32, i32, c_f, c_f, i32, c_f, c_f, c_f, i64, f32, c_f, i64, i64, c_f, c_f, C.c_void_p]),
+    "b2a_vocos_istft_head": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, i64, C.c_void_p]),
+    "b2a_vocos_logmel": (i32, [c_f, i64, i32, i64, c_f, c_f, i32, i64, c_f, C.c_void_p]),
 }
 
 E_INVALID, E_CUDA, E_UNSUPPORTED = -1, -2, -3

@@ -55,3 +55,20 @@ QWEN3_TOKENIZER_ENCODER = {      # the speech-tokenizer encoder (ICL voice cloni
     "num_heads": 8, "num_layers": 8, "dim_feedforward": 2048, "context": 250, "max_period": 10000, "layer_scale": 0.01, "nq": 32, "bins": 2048,
     "qdim": 256, "upsample_stride": 2, "valid_num_quantizers": 16,
 }
+
+
+# Vocos (codec/tests/test_vocos.py config_mel / config_encodec): the released 24 kHz mel checkpoint and the EnCodec-feature one, in the
+# YAML shape Vocos.from_hparams takes.
+VOCOS_MEL_24K = {
+    "feature_extractor": {"class_path": "vocos.feature_extractors.MelSpectrogramFeatures",
+                          "init_args": {"sample_rate": 24000, "n_fft": 1024, "hop_length": 256, "n_mels": 100}},
+    "backbone": {"class_path": "vocos.models.VocosBackbone", "init_args": {"input_channels": 100, "dim": 512, "intermediate_dim": 1536, "num_layers": 8}},
+    "head": {"class_path": "vocos.heads.ISTFTHead", "init_args": {"dim": 512, "n_fft": 1024, "hop_length": 256}},
+}
+VOCOS_ENCODEC_24K = {
+    "feature_extractor": {"class_path": "vocos.feature_extractors.EncodecFeatures",
+                          "init_args": {"encodec_model": "encodec_24khz", "bandwidths": [1.5, 3.0, 6.0, 12.0, 24.0]}},
+    "backbone": {"class_path": "vocos.models.VocosBackbone",
+                 "init_args": {"input_channels": 128, "dim": 384, "intermediate_dim": 1152, "num_layers": 8, "adanorm_num_embeddings": 4}},
+    "head": {"class_path": "vocos.heads.ISTFTHead", "init_args": {"dim": 384, "n_fft": 1280, "hop_length": 320, "padding": "same"}},
+}

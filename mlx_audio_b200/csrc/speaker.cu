@@ -4,61 +4,12 @@
 // run on the tensor-core conv, everything between them is here.
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "spk_logmel.cuh"
 
 namespace {
 
-// ---------------------------------------------------------------- log-mel front end
-constexpr int MEL_FT = 8;          // frames per CTA
-constexpr int MEL_N = 1024, MEL_HOP = 256, MEL_NF = MEL_N / 2 + 1, MEL_PAD = (MEL_N - MEL_HOP) / 2;
-
-// One CTA = MEL_FT frames of one item: reflect-padded (by MEL_PAD samples, no repeated edge) windowed frames, direct DFT against an
-// exact twiddle table (index (k*i) mod N, no accumulated angle), sqrt(|X|^2 + 1e-9), Slaney mel projection, log(max(., 1e-5)).
-__global__ void spk_logmel_kernel(const float* __restrict__ x, int64_t x_bs, int64_t n, const float* __restrict__ window,
-                                  const float* __restrict__ filters, int n_mels, int64_t frames, float* __restrict__ out) {
-  extern __shared__ __align__(16) float sm[];
-  float* tw_c = sm;
-  float* tw_s = sm + MEL_N;
-  float* fr = sm + 2 * MEL_N;                 // [MEL_FT][MEL_N]
-  float* mag = fr + MEL_FT * MEL_N;           // [MEL_FT][MEL_NF]
-  const int b = blockIdx.y;
-  const int64_t f0 = (int64_t)blockIdx.x * MEL_FT;
-  const float* xb = x + (int64_t)b * x_bs;
-  for (int i = threadIdx.x; i < MEL_N; i += blockDim.x) { float s, c; sincospif(2.f * i / MEL_N, &s, &c); tw_c[i] = c; tw_s[i] = s; }
-  for (int idx = threadIdx.x; idx < MEL_FT * MEL_N; idx += blockDim.x) {
-    const int f = idx / MEL_N, i = idx % MEL_N;
-    float v = 0.f;
-    if (f0 + f < frames) {
-      int64_t s = (f0 + f) * MEL_HOP + i - MEL_PAD;          // position in the unpadded signal
-      if (s < 0) s = -s;
-      else if (s >= n) s = 2 * (n - 1) - s;
-      v = __ldg(xb + s) * __ldg(window + i);
-    }
-    fr[idx] = v;
-  }
-  __syncthreads();
-  for (int idx = threadIdx.x; idx < MEL_FT * MEL_NF; idx += blockDim.x) {
-    const int f = idx / MEL_NF, k = idx % MEL_NF;
-    const float* xr = fr + f * MEL_N;
-    float re = 0.f, im = 0.f;
-    int ph = 0;
-    for (int i = 0; i < MEL_N; i++) {
-      re = fmaf(xr[i], tw_c[ph], re);
-      im = fmaf(-xr[i], tw_s[ph], im);
-      ph = (ph + k) & (MEL_N - 1);
-    }
-    mag[idx] = sqrtf(re * re + im * im + 1e-9f);
-  }
-  __syncthreads();
-  for (int idx = threadIdx.x; idx < MEL_FT * n_mels; idx += blockDim.x) {
-    const int f = idx / n_mels, m = idx % n_mels;
-    if (f0 + f >= frames) continue;
-    const float* fl = filters + (int64_t)m * MEL_NF;
-    const float* mr = mag + f * MEL_NF;
-    float acc = 0.f;
-    for (int k = 0; k < MEL_NF; k++) acc = fmaf(mr[k], __ldg(fl + k), acc);
-    out[((int64_t)b * frames + f0 + f) * n_mels + m] = logf(fmaxf(acc, 1e-5f));
-  }
-}
+// ---------------------------------------------------------------- log-mel front end (spk_logmel.cuh): centre pad 384, |X| with 1e-9
+constexpr int MEL_PAD = (MEL_N - MEL_HOP) / 2;
 
 // ---------------------------------------------------------------- reflect "same" padding as the operand of the next conv
 __device__ __forceinline__ int reflect_idx(int q, int T) {
@@ -362,11 +313,11 @@ extern "C" int32_t b2a_spk_logmel(const float* x, int64_t x_bs, int32_t B, int64
   B2A_CHECK_ARG(x && window && filters && out && B > 0 && n_mels > 0 && frames > 0, "bad pointers/shape");
   B2A_CHECK_ARG(n > MEL_PAD, "reflect padding needs more than 384 samples");
   B2A_CHECK_ARG(frames == 1 + (n + 2 * MEL_PAD - MEL_N) / MEL_HOP, "frames must be 1 + (n + 768 - 1024) / 256");
-  const size_t smem = (size_t)(2 * MEL_N + MEL_FT * MEL_N + MEL_FT * MEL_NF) * sizeof(float);
+  const size_t smem = spk_logmel_smem_bytes();
   static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(spk_logmel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+  if (!attr) { cudaFuncSetAttribute(spk_logmel_kernel<MEL_PAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
   dim3 grid(cdiv(frames, MEL_FT), B);
-  spk_logmel_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(x, x_bs, n, window, filters, n_mels, frames, out);
+  spk_logmel_kernel<MEL_PAD, true><<<grid, 256, smem, (cudaStream_t)stream>>>(x, x_bs, n, window, filters, n_mels, frames, out);
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }

@@ -1458,3 +1458,58 @@ def spk_asp_pool(logits: torch.Tensor, x: torch.Tensor, eps: float = 1e-12) -> t
     _call("other", _lib.lib().b2a_spk_asp_pool, 1, logits.data_ptr(), logits.stride(0), logits.stride(1), x.data_ptr(), x.stride(0),
           x.stride(1), B, T, Cc, eps, out.data_ptr(), out.stride(0), _stream())
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------- Vocos
+def vocos_dwnorm(x: torch.Tensor, dw: Optional[ConvW], w: Optional[torch.Tensor], b: Optional[torch.Tensor], *, ada: Optional[torch.Tensor] = None,
+                 eps: float = 1e-6, fp32: bool = True, planes: bool = False):
+    """Vocos's ConvNeXt dwconv + LayerNorm / AdaLayerNorm (vocos.py:183-187) in one launch; ``dw`` None: the norm alone (the backbone's
+    norm and final_layer_norm).  x [B, L, C]; ``dw`` a depthwise ``pack_conv`` (odd K <= 15); affine ``w`` / ``b`` (either may be None),
+    or ``ada`` [B, 2C] rows (scale | shift, row stride free) applied as scale v + shift.  Returns fp32 [B, L, C] (``fp32``), the next
+    GEMM's bf16 ``Planes`` [B, L, C] (``planes``, C % 64 == 0), or (y, planes) with both."""
+    _chk3(x, "vocos_dwnorm x")
+    B, L, Cc = x.shape
+    if not (fp32 or planes):
+        raise ValueError("vocos_dwnorm: ask for fp32 rows, planes or both")
+    if dw is not None and (dw.groups != Cc or dw.cin != Cc or dw.K % 2 == 0 or dw.K > 15):
+        raise ValueError("vocos_dwnorm: dw must be a depthwise conv over x's channels with an odd number of taps <= 15")
+    if ada is not None and (ada.dim() != 2 or ada.shape[0] != B or ada.shape[1] != 2 * Cc or ada.stride(1) != 1 or ada.dtype != torch.float32):
+        raise ValueError(f"vocos_dwnorm: ada must be float32 [B, 2C] = {(B, 2 * Cc)} rows with unit column stride")
+    y = torch.empty(B, L, Cc, device=x.device, dtype=torch.float32) if fp32 else None
+    pl = _new_planes(B, L, Cc, x.device) if planes else None
+    _call("vocos_norm", _lib.lib().b2a_vocos_dwnorm, 1, x.data_ptr(), x.stride(0), x.stride(1), B, L, Cc,
+          None if dw is None else dw.w.data_ptr(), None if dw is None else _p(dw.bias), 0 if dw is None else dw.K, _p(w), _p(b), _p(ada),
+          0 if ada is None else ada.stride(0), float(eps), _p(y), 0 if y is None else y.stride(0), 0 if y is None else y.stride(1),
+          None if pl is None else pl.hi.data_ptr(), None if pl is None else _p(pl.lo), _stream())
+    if fp32 and planes:
+        return y, pl
+    return y if fp32 else pl
+
+
+def vocos_istft_head(h: torch.Tensor, n_fft: int, hop: int, window: torch.Tensor) -> torch.Tensor:
+    """ISTFTHead after its linear (vocos.py:126-140, dsp.py:436-513): h [B, T, ld >= n_fft + 2] (log-magnitude | phase columns; any
+    columns beyond n_fft + 2 are ignored) -> waveform [B, (T - 1) * hop].  ``window``: the symmetric Hann window [n_fft]."""
+    _chk3(h, "vocos_istft_head h")
+    B, T, ld = h.shape
+    if ld < n_fft + 2 or window.numel() != n_fft or window.dtype != torch.float32 or not window.is_contiguous():
+        raise ValueError(f"vocos_istft_head: needs h rows of >= {n_fft + 2} columns and a contiguous float32 window of {n_fft}")
+    out = torch.empty(B, (T - 1) * hop, device=h.device, dtype=torch.float32)
+    if T > 1:
+        _call("vocos_head", _lib.lib().b2a_vocos_istft_head, 1, h.data_ptr(), h.stride(0), h.stride(1), B, T, n_fft, hop, window.data_ptr(),
+              out.data_ptr(), out.stride(0), _stream())
+    return out
+
+
+def vocos_logmel(x: torch.Tensor, window: torch.Tensor, filters: torch.Tensor) -> torch.Tensor:
+    """Vocos's log-mel (mel.py:8-33) at n_fft 1024 / hop 256: x [B, n] float32 -> [B, n // 256, n_mels]; ``window`` the symmetric Hann
+    window [1024], ``filters`` HTK mel filters [n_mels, 513]."""
+    B, n = x.shape
+    if x.dtype != torch.float32 or x.stride(1) != 1 or window.numel() != 1024 or not filters.is_contiguous() or filters.shape[1] != 513:
+        raise ValueError("vocos_logmel: x [B, n] float32 with unit stride, a 1024-sample window and [n_mels, 513] filters")
+    if n <= 512:
+        raise ValueError(f"vocos log-mel: the reflect padding of 512 samples needs more than 512 samples, got {n}")
+    frames = n // 256
+    out = torch.empty(B, frames, filters.shape[0], device=x.device, dtype=torch.float32)
+    _call("logmel", _lib.lib().b2a_vocos_logmel, 1, x.data_ptr(), x.stride(0), B, n, window.data_ptr(), filters.data_ptr(), filters.shape[0],
+          frames, out.data_ptr(), _stream())
+    return out

@@ -660,3 +660,47 @@ def qwen3_speaker_encoder_weights(cfg, seed=14):
     conv(p + "asp.conv", ch[-1], 1, A)
     conv(p + "fc", E, 1, 2 * ch[-1])
     return g.P
+
+
+def vocos_backbone_weights(bb, seed=11, prefix="backbone."):
+    """MLX-layout parameters of a ``codec.models.vocos.VocosBackbone``: convs and linears ~ N(0, 1/fan_in) (unit gain), biases 0.05 N(0, 1),
+    LayerNorm gains 1 + 0.1 N(0, 1); AdaLayerNorm's scale linear gives 1 + small per condition (weights 0.1 / E N(0, 1), bias 1), its shift
+    linear small values; ``gamma`` the constructor's value.  bf16-exact weights, so the tensor-core path holds them exactly."""
+    g = _Gen(seed)
+    for name, shape in bb.param_shapes(prefix).items():
+        leaf = name.rsplit(".", 1)[-1]
+        if leaf == "gamma":
+            g.const(name, bb.layer_scale_init_value, *shape)
+        elif ".scale." in name or ".shift." in name:
+            g.normal(name, *shape, std=0.1 / shape[-1] if leaf == "weight" else 0.05)
+            if name.endswith(".scale.bias"):
+                g.P[name] = g.P[name] + 1.0
+        elif leaf == "bias":
+            g.normal(name, *shape, std=0.05)
+        elif len(shape) == 1:
+            g.P[name] = _bf16(1.0 + 0.1 * torch.randn(*shape, generator=g.g))
+        else:
+            _fan(g, name, *shape, fan_in=math.prod(shape[1:]))
+    return g.P
+
+
+def vocos_head_weights(head, seed=12, prefix="head."):
+    """ISTFTHead's linear at unit gain: its input is LayerNorm output (~unit variance), so the log-magnitudes are ~N(-0.5, 1) and well under
+    1 % of the bins reach exp(.) > 100 -- the clip does not hide errors -- and the phases ~N(0, 1)."""
+    g = _Gen(seed)
+    (wn, ws), (bn, bs) = head.param_shapes(prefix).items()
+    _fan(g, wn, *ws, fan_in=ws[1])
+    b = 0.05 * torch.randn(*bs, generator=g.g)
+    b[: head.n_fft // 2 + 1] -= 0.5
+    g.P[bn] = _bf16(b)
+    return g.P
+
+
+def vocos_weights(config: dict, seed=11) -> dict:
+    """Released-size synthetic parameters for ``Vocos.from_hparams(config)`` (the reference's YAML-shaped dict)."""
+    from .codec.models.vocos import ISTFTHead, VocosBackbone
+    bb = VocosBackbone(**config["backbone"]["init_args"], device="cpu")
+    hd = ISTFTHead(**config["head"]["init_args"], device="cpu")
+    P = vocos_backbone_weights(bb, seed)
+    P.update(vocos_head_weights(hd, seed + 1))
+    return P
