@@ -595,6 +595,37 @@ int32_t b2a_vocos_istft_head(const float* h, int64_t h_bs, int64_t h_ld, int32_t
 int32_t b2a_vocos_logmel(const float* x, int64_t x_bs, int32_t B, int64_t n, const float* window, const float* filters, int32_t n_mels,
                          int64_t frames, float* out, void* stream);
 
+/* ---- EnCodec (encodec.cu; codec/models/encodec/encodec.py) --------------------------------------------------------------------
+ * One unidirectional LSTM layer (encodec.py:89-169) over xproj [R, T, 4H] contiguous (x Wx^T + bias, gates i, f, g, o), W_h [4H, H]
+ * fp32; h0 = c0 = 0.  out [R, T, H] contiguous = h, plus skip [R, T, H] (or NULL) -- EncodecLSTM's residual on its last layer.  One
+ * cluster of H / 32 CTAs per 4 rows (1 for R == 1); a row's result does not depend on R.  H in {128, 256, 512}, else B2A_E_UNSUPPORTED,
+ * as is a device that cannot schedule the cluster.  `err` (uint32, zeroed by the caller) is set to 1 when a step waited more than 10 s
+ * (that call's output is then invalid). */
+int32_t b2a_encodec_lstm(const float* xproj, const float* wh, const float* skip, float* out, int32_t R, int32_t T, int32_t H, uint32_t* err,
+                         void* stream);
+/* The input side of EncodecConv1d (encodec.py:212-245): y [B, pad_left + T + pad_right, C] from x [B, T, C] (strides x_bs, x_ld; y_bs,
+ * y_ld) with reflect (no repeated edge; pad_left, pad_right < T, else B2A_E_INVALID) or zero padding.  Each source value first gets
+ * v * scale[b, C] + shift[b, C] (both or neither NULL: a GroupNorm applied from b2a_encodec_gn_coeffs) and then ELU when `elu`; zero
+ * padding stays 0.  res (or NULL; strides res_bs, res_ld) is added afterwards and requires pad_left == pad_right == 0. */
+int32_t b2a_encodec_pad(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T, int32_t C, int32_t pad_left, int32_t pad_right,
+                        int32_t reflect, const float* scale, const float* shift, int32_t elu, const float* res, int64_t res_bs, int64_t res_ld,
+                        float* y, int64_t y_bs, int64_t y_ld, void* stream);
+/* GroupNorm(1, C) (MLX, pytorch_compatible) of x [B, T, C]: mean and biased variance over T x C per row in float64 with a fixed order
+ * (independent of B), folded with gamma / beta [C] (NULL: 1 / 0) into scale[b, c] = gamma rstd, shift[b, c] = beta - mean gamma rstd
+ * ([B, C] contiguous).  ws: b2a_encodec_gn_ws_bytes(B) bytes of device memory.  Two launches. */
+int64_t b2a_encodec_gn_ws_bytes(int32_t B);
+int32_t b2a_encodec_gn_coeffs(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t T, int32_t C, const float* gamma,
+                              const float* beta, float eps, float* scale, float* shift, void* ws, void* stream);
+/* Encodec._encode_frame's normalisation (encodec.py:574-579) per chunk row r of x [R, L, C]: v = x * mask[r, t] (mask uint8 with row
+ * stride mask_bs, or NULL), scale[r] = sqrt(mean_t(mean_c v)^2) + 1e-8 (float64 sums), y [R, L, C] contiguous = v / scale[r]. */
+int32_t b2a_encodec_normalize(const float* x, int64_t x_bs, int64_t x_ld, int32_t R, int32_t L, int32_t C, const uint8_t* mask,
+                              int64_t mask_bs, float* y, float* scale, void* stream);
+/* Encodec._linear_overlap_add (encodec.py:654-677) of N chunk decodes frames [N, B, L, C] contiguous, each first multiplied by
+ * scale[n * B + b] (or NULL), at `stride` <= L, with the triangular weight 0.5 - |(j + 1) / (L + 1) - 0.5|, divided by the summed
+ * weights and truncated: out [B, Tout, C] contiguous, Tout <= stride (N - 1) + L.  Chunks summed in ascending order. */
+int32_t b2a_encodec_ola(const float* frames, int32_t N, int32_t B, int32_t L, int32_t C, const float* scale, int32_t stride, int32_t Tout,
+                        float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

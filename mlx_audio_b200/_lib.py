@@ -165,6 +165,12 @@ PROTOTYPES = {
     "b2a_vocos_dwnorm": (i32, [c_f, i64, i64, i32, i32, i32, c_f, c_f, i32, c_f, c_f, c_f, i64, f32, c_f, i64, i64, c_f, c_f, C.c_void_p]),
     "b2a_vocos_istft_head": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, i64, C.c_void_p]),
     "b2a_vocos_logmel": (i32, [c_f, i64, i32, i64, c_f, c_f, i32, i64, c_f, C.c_void_p]),
+    "b2a_encodec_lstm": (i32, [c_f, c_f, c_f, c_f, i32, i32, i32, c_f, C.c_void_p]),
+    "b2a_encodec_pad": (i32, [c_f, i64, i64, i32, i32, i32, i32, i32, i32, c_f, c_f, i32, c_f, i64, i64, c_f, i64, i64, C.c_void_p]),
+    "b2a_encodec_gn_ws_bytes": (i64, [i32]),
+    "b2a_encodec_gn_coeffs": (i32, [c_f, i64, i64, i32, i32, i32, c_f, c_f, f32, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_encodec_normalize": (i32, [c_f, i64, i64, i32, i32, i32, c_f, i64, c_f, c_f, C.c_void_p]),
+    "b2a_encodec_ola": (i32, [c_f, i32, i32, i32, i32, c_f, i32, i32, c_f, C.c_void_p]),
 }
 
 E_INVALID, E_CUDA, E_UNSUPPORTED = -1, -2, -3

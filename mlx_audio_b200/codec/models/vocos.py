@@ -11,7 +11,10 @@ Kept from the reference: the backbone transposes its input when ``x.shape[-1] !=
 taken as [B, T, C]); the head's and the feature extractor's ``padding`` are ignored; ``gamma`` defaults to ``layer_scale_init_value or
 1 / num_layers``.  Extension: B > 1 everywhere (the reference's head squeezes axis 0); B = 1 returns the reference's 1-D waveform, B > 1
 returns [B, samples].  Divergences: audio of <= n_fft // 2 samples raises ``ValueError`` (the reference's reflect pad silently builds a short
-pad); only the released mel front end (n_fft 1024, hop 256) runs on the GPU; EnCodec features need EnCodec, which this package does not have.
+pad); only the released mel front end (n_fft 1024, hop 256) runs on the GPU; ``EncodecFeatures`` never loads an EnCodec model by itself
+(the reference downloads one from the hub when it is constructed): audio input and ``decode_from_codes`` work once a model is attached
+with ``encodec=`` (an ``Encodec`` or a local checkpoint directory) on ``EncodecFeatures``, ``from_hparams`` or ``from_pretrained``, and
+raise ``NotImplementedError`` otherwise; ``decode(features, bandwidth_id=...)`` works either way.
 """
 from __future__ import annotations
 
@@ -84,17 +87,62 @@ class MelSpectrogramFeatures:
 
 
 class EncodecFeatures:
-    """vocos.py:54-116 needs the EnCodec model, which this package does not have: constructing it is fine (``from_hparams`` on an EnCodec
-    config builds the backbone and head, so ``decode(features, bandwidth_id=...)`` works), using it raises."""
+    """vocos.py:54-116 on an EnCodec model attached explicitly (``encodec=``: an ``Encodec``, or a local directory for
+    ``Encodec.from_pretrained``).  Constructing one without a model builds nothing (``from_hparams`` on an EnCodec config builds the
+    backbone and head, so ``decode(features, bandwidth_id=...)`` works); using it then raises ``NotImplementedError``."""
 
-    def __init__(self, encodec_model="encodec_24khz", bandwidths=(1.5, 3.0, 6.0, 12.0), train_codebooks=False, **_):
+    def __init__(self, encodec_model="encodec_24khz", bandwidths=(1.5, 3.0, 6.0, 12.0), train_codebooks=False, encodec=None, device="cuda", **_):
+        if encodec_model not in ("encodec_24khz", "encodec_48khz"):
+            raise ValueError(f"Unsupported encodec_model: {encodec_model}. Supported options are 'encodec_24khz' and 'encodec_48khz'.")
         self.encodec_model, self.bandwidths = encodec_model, list(bandwidths)
+        self.encodec = self.preprocessor = None
+        if encodec is not None:
+            self.attach(encodec, device)
 
-    def _missing(self, *_a, **_k):
-        raise NotImplementedError("Vocos EncodecFeatures needs the EnCodec model, which mlx_audio_b200 does not provide; "
-                                  "decode(features, bandwidth_id=...) with precomputed features works")
+    def attach(self, encodec, device="cuda"):
+        """Use ``encodec`` (an ``Encodec`` or a local checkpoint directory) as this extractor's model."""
+        from .encodec import Encodec, preprocess_audio
+        import functools
+        if isinstance(encodec, Encodec):
+            self.encodec = encodec
+            self.preprocessor = functools.partial(preprocess_audio, sampling_rate=encodec.sampling_rate, chunk_length=encodec.chunk_length,
+                                                  chunk_stride=encodec.chunk_stride, device=encodec.device)
+        else:
+            self.encodec, self.preprocessor = Encodec.from_pretrained(encodec, device=device)
+        self.num_q = self.encodec.get_num_quantizers_for_bandwidth(max(self.bandwidths))
+        return self
 
-    __call__ = get_encodec_codes = get_features_from_codes = _missing
+    def _need(self):
+        if self.encodec is None:
+            raise NotImplementedError("Vocos EncodecFeatures: no EnCodec model attached; pass encodec=<Encodec or local directory> to "
+                                      "EncodecFeatures / Vocos.from_hparams / Vocos.from_pretrained (decode(features, bandwidth_id=...) "
+                                      "with precomputed features works without one)")
+
+    def get_encodec_codes(self, audio, bandwidth_id):
+        """audio [n] -> codes int64 [nq, 1, T] at ``bandwidths[bandwidth_id]`` (a list or tensor id: its first entry, as the reference)."""
+        self._need()
+        features, mask = self.preprocessor(audio)
+        if isinstance(bandwidth_id, (torch.Tensor, np.ndarray)):
+            bandwidth_id = int(np.asarray(torch.as_tensor(bandwidth_id).cpu()).reshape(-1)[0])
+        elif isinstance(bandwidth_id, (list, tuple)):
+            bandwidth_id = bandwidth_id[0]
+        codes, _ = self.encodec.encode(features, mask, bandwidth=self.bandwidths[int(bandwidth_id)])
+        return codes.reshape(codes.shape[-2], 1, codes.shape[-1])
+
+    def get_features_from_codes(self, codes):
+        """codes [nq <= num_q, B, T] -> the sum of their code vectors [B, T, codebook_dim] (one rvq_decode)."""
+        self._need()
+        codes = torch.as_tensor(np.asarray(codes) if not isinstance(codes, torch.Tensor) else codes).to(self.encodec.device, torch.int64)
+        if codes.dim() != 3 or not 1 <= codes.shape[0] <= self.num_q:
+            raise ValueError(f"EncodecFeatures: codes must be [1..{self.num_q}, B, T], got {tuple(codes.shape)}")
+        return self.encodec._dequantize(codes.permute(1, 0, 2))
+
+    def __call__(self, audio, **kwargs):
+        self._need()
+        bandwidth_id = kwargs.get("bandwidth_id")
+        if bandwidth_id is None:
+            raise ValueError("The 'bandwidth_id' argument is required")
+        return self.get_features_from_codes(self.get_encodec_codes(audio, bandwidth_id))
 
 
 class VocosBackbone:
@@ -261,12 +309,13 @@ class Vocos:
         self.feature_extractor, self.backbone, self.head = feature_extractor, backbone, head
 
     @classmethod
-    def from_hparams(cls, config: dict, device="cuda") -> "Vocos":
+    def from_hparams(cls, config: dict, device="cuda", encodec=None) -> "Vocos":
+        """``encodec``: the EnCodec model (or local directory) an ``EncodecFeatures`` extractor uses; nothing is loaded without it."""
         fe_cfg = config["feature_extractor"]
         if "MelSpectrogramFeatures" in fe_cfg["class_path"]:
             fe = MelSpectrogramFeatures(**fe_cfg.get("init_args", {}), device=device)
         elif "EncodecFeatures" in fe_cfg["class_path"]:
-            fe = EncodecFeatures(**fe_cfg.get("init_args", {}))
+            fe = EncodecFeatures(**fe_cfg.get("init_args", {}), encodec=encodec, device=device)
         else:
             raise ValueError(f"Vocos: unknown feature extractor {fe_cfg['class_path']!r}")
         return cls(fe, VocosBackbone(**config["backbone"]["init_args"], device=device), ISTFTHead(**config["head"]["init_args"], device=device))
@@ -297,7 +346,7 @@ class Vocos:
         return self
 
     @classmethod
-    def from_pretrained(cls, path_or_repo: str, device="cuda") -> "Vocos":
+    def from_pretrained(cls, path_or_repo: str, device="cuda", encodec=None) -> "Vocos":
         """vocos.py:307-354 for a LOCAL directory (config.yaml + model.safetensors); a hub id is resolved through huggingface_hub only
         when that package can reach it."""
         import yaml
@@ -308,7 +357,7 @@ class Vocos:
             path = Path(snapshot_download(repo_id=path_or_repo, allow_patterns=["*.yaml", "*.safetensors"]))
         with open(path / "config.yaml") as f:
             config = yaml.safe_load(f)
-        model = cls.from_hparams(config, device=device)
+        model = cls.from_hparams(config, device=device, encodec=encodec)
         return model.load_weights(cls.sanitize(load_file(str(path / "model.safetensors"))))
 
     @torch.no_grad()

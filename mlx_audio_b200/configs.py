@@ -72,3 +72,14 @@ VOCOS_ENCODEC_24K = {
                  "init_args": {"input_channels": 128, "dim": 384, "intermediate_dim": 1152, "num_layers": 8, "adanorm_num_embeddings": 4}},
     "head": {"class_path": "vocos.heads.ISTFTHead", "init_args": {"dim": 384, "n_fft": 1280, "hop_length": 320, "padding": "same"}},
 }
+
+
+# EnCodec (mlx-community/encodec-{24,48}khz-float32 config.json): 24 kHz mono, causal, weight norm; 48 kHz stereo, non-causal,
+# time_group_norm, normalize, 1 s chunks with 1 % overlap.  Encodec(config) takes either dict.
+ENCODEC_24K = dict(model_type="encodec", audio_channels=1, num_filters=32, kernel_size=7, num_residual_layers=1, dilation_growth_rate=2,
+                   codebook_size=1024, codebook_dim=128, hidden_size=128, num_lstm_layers=2, residual_kernel_size=3, use_causal_conv=True,
+                   normalize=False, pad_mode="reflect", norm_type="weight_norm", last_kernel_size=7, trim_right_ratio=1.0, compress=2,
+                   upsampling_ratios=[8, 5, 4, 2], target_bandwidths=[1.5, 3.0, 6.0, 12.0, 24.0], sampling_rate=24000,
+                   chunk_length_s=None, overlap=None)
+ENCODEC_48K = dict(ENCODEC_24K, audio_channels=2, use_causal_conv=False, normalize=True, norm_type="time_group_norm",
+                   target_bandwidths=[3.0, 6.0, 12.0, 24.0], sampling_rate=48000, chunk_length_s=1.0, overlap=0.01)

@@ -1513,3 +1513,73 @@ def vocos_logmel(x: torch.Tensor, window: torch.Tensor, filters: torch.Tensor) -
     _call("logmel", _lib.lib().b2a_vocos_logmel, 1, x.data_ptr(), x.stride(0), B, n, window.data_ptr(), filters.data_ptr(), filters.shape[0],
           frames, out.data_ptr(), _stream())
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------- EnCodec
+def encodec_lstm(xproj: torch.Tensor, wh: torch.Tensor, err: torch.Tensor, skip: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One unidirectional LSTM layer (encodec.py:89-169): xproj [R, T, 4H] (x Wx^T + bias), wh [4H, H] -> h [R, T, H] (+ ``skip``).
+    ``err``: int32 [1] on the device, set to 1 by a step that waited more than 10 s (checked by the caller)."""
+    R, T, g4 = xproj.shape
+    H = g4 // 4
+    for name, t in (("xproj", xproj), ("wh", wh)) + ((("skip", skip),) if skip is not None else ()):
+        if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+            raise ValueError(f"encodec_lstm: {name} must be a contiguous CUDA float32 tensor")
+    if tuple(wh.shape) != (4 * H, H) or (skip is not None and tuple(skip.shape) != (R, T, H)):
+        raise ValueError(f"encodec_lstm: wh must be [{4 * H}, {H}] and skip [{R}, {T}, {H}]")
+    out = torch.empty(R, T, H, device=xproj.device, dtype=torch.float32)
+    _call("lstm", _lib.lib().b2a_encodec_lstm, 1, xproj.data_ptr(), wh.data_ptr(), _p(skip), out.data_ptr(), R, T, H, err.data_ptr(), _stream())
+    return out
+
+
+def encodec_pad(x: torch.Tensor, pad_left: int, pad_right: int, *, reflect: bool = True, coeffs=None, elu: bool = False,
+                res: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """EncodecConv1d's input side: x [B, T, C] (row-strided views allowed) -> fp32 [B, pad_left + T + pad_right, C]; each source value
+    gets the GroupNorm ``coeffs`` = (scale, shift) [B, C] and then ELU first; ``res`` [B, T, C] is added last (no padding then)."""
+    _chk3(x, "encodec_pad x")
+    B, T, Cc = x.shape
+    if reflect and max(pad_left, pad_right) >= T:
+        raise ValueError(f"EnCodec reflect padding ({pad_left}, {pad_right}) needs more than {max(pad_left, pad_right)} frames, got {T}")
+    out = torch.empty(B, pad_left + T + pad_right, Cc, device=x.device, dtype=torch.float32)
+    sc, sh = coeffs if coeffs is not None else (None, None)
+    if res is not None:
+        _chk3(res, "encodec_pad res")
+    _call("prep", _lib.lib().b2a_encodec_pad, 1, x.data_ptr(), x.stride(0), x.stride(1), B, T, Cc, pad_left, pad_right, int(reflect), _p(sc),
+          _p(sh), int(elu), _p(res), 0 if res is None else res.stride(0), 0 if res is None else res.stride(1), out.data_ptr(), out.stride(0),
+          out.stride(1), _stream())
+    return out
+
+
+def encodec_gn_coeffs(x: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor], eps: float = 1e-5):
+    """GroupNorm(1, C) of x [B, T, C] folded with its affine -> (scale, shift) [B, C] float32 for ``encodec_pad(coeffs=)``."""
+    _chk3(x, "encodec_gn_coeffs x")
+    B, T, Cc = x.shape
+    scale = torch.empty(B, Cc, device=x.device, dtype=torch.float32)
+    shift = torch.empty(B, Cc, device=x.device, dtype=torch.float32)
+    ws = _workspace(_lib.lib().b2a_encodec_gn_ws_bytes(B), x.device)
+    _call("norm", _lib.lib().b2a_encodec_gn_coeffs, 2, x.data_ptr(), x.stride(0), x.stride(1), B, T, Cc, _p(gamma), _p(beta), eps,
+          scale.data_ptr(), shift.data_ptr(), ws.data_ptr(), _stream())
+    return scale, shift
+
+
+def encodec_normalize(x: torch.Tensor, mask: Optional[torch.Tensor]):
+    """Per chunk row of x [R, L, C]: (x * mask / scale, scale [R]) with scale = RMS of the masked mono mix + 1e-8 (encodec.py:574-579)."""
+    _chk3(x, "encodec_normalize x")
+    R, L, Cc = x.shape
+    if mask is not None:
+        assert mask.dtype in (torch.bool, torch.uint8) and tuple(mask.shape) == (R, L) and mask.stride(1) == 1
+    y = torch.empty(R, L, Cc, device=x.device, dtype=torch.float32)
+    scale = torch.empty(R, device=x.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_encodec_normalize, 1, x.data_ptr(), x.stride(0), x.stride(1), R, L, Cc, _p(mask),
+          0 if mask is None else mask.stride(0), y.data_ptr(), scale.data_ptr(), _stream())
+    return y, scale
+
+
+def encodec_ola(frames: torch.Tensor, B: int, scale: Optional[torch.Tensor], stride: int, t_out: int) -> torch.Tensor:
+    """Encodec._linear_overlap_add (encodec.py:654-677) of chunk decodes frames [N * B, L, C] (chunk-major), each times scale [N * B]
+    (or None), truncated to ``t_out`` samples -> [B, t_out, C]."""
+    NB, L, Cc = frames.shape
+    assert frames.dtype == torch.float32 and frames.is_contiguous() and NB % B == 0
+    assert scale is None or (scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == NB)
+    out = torch.empty(B, t_out, Cc, device=frames.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_encodec_ola, 1, frames.data_ptr(), NB // B, B, L, Cc, _p(scale), stride, t_out, out.data_ptr(), _stream())
+    return out

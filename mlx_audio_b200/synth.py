@@ -704,3 +704,31 @@ def vocos_weights(config: dict, seed=11) -> dict:
     P = vocos_backbone_weights(bb, seed)
     P.update(vocos_head_weights(hd, seed + 1))
     return P
+
+
+def encodec_weights(config: dict, seed=15) -> dict:
+    """MLX-layout parameters of ``codec.models.encodec.Encodec(config)`` (float32, as the released checkpoints are): convs ~ N(0, 1/fan_in)
+    (unit gain; the residual branch's last conv and the shortcut at 1/sqrt(2) so that a block keeps the scale), biases N(0, 0.05^2),
+    GroupNorm gains 1 + 0.1 N(0, 1); LSTM Wx and Wh ~ N(0, 0.5^2 / H), bias N(0, 0.1^2) -- gate pre-activations of order 1, neither
+    saturated nor vanishing; code book q: rows of nearly equal norm (so that the nearest code is decided by direction and every code is
+    used), 0.15 * 0.8^q per element, shrinking with the residual it quantises."""
+    from .codec.models.encodec import param_shapes
+    g = torch.Generator().manual_seed(seed)
+    P = {}
+    for name, shape in param_shapes(config).items():
+        leaf = name.rsplit(".", 1)[-1]
+        if leaf == "embed":
+            q = int(name.split(".")[2])
+            e = torch.randn(*shape, generator=g)
+            e = e / e.norm(dim=1, keepdim=True) * math.sqrt(shape[1]) * (1 + 0.05 * torch.randn(shape[0], 1, generator=g))
+            P[name] = 0.15 * 0.8 ** q * e
+        elif leaf in ("Wx", "Wh"):
+            P[name] = 0.5 / math.sqrt(shape[1]) * torch.randn(*shape, generator=g)
+        elif leaf == "bias":
+            P[name] = (0.1 if name.endswith(("Wx", "lstm")) or ".lstm." in name else 0.05) * torch.randn(*shape, generator=g)
+        elif ".norm." in name:
+            P[name] = 1.0 + 0.1 * torch.randn(*shape, generator=g)
+        else:
+            gain = 1 / math.sqrt(2) if (".block.3." in name or ".shortcut." in name) else 1.0
+            P[name] = gain / math.sqrt(shape[1] * shape[2]) * torch.randn(*shape, generator=g)
+    return P
