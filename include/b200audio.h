@@ -299,6 +299,10 @@ typedef struct {
 } b2a_convf_t;
 int32_t b2a_conv1d_fused_debug(void* stamps /* device uint64 [grid][16] or NULL: phase time stamps of the next launches */);
 int32_t b2a_conv1d_fused(const b2a_convf_t* problems, int32_t n_problems, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream);
+/* 1 when a launch of one problem with taps spanning `span` rows (0..64), N GEMM columns over C output channels (N = up_stride * C in
+ * polyphase mode, else N = C), wplanes weight planes (2: w_lo set) and `planes` activation planes finds room for two weight stages in
+ * shared memory, else 0 (b2a_conv1d_fused would return B2A_E_UNSUPPORTED).  Host-side only. */
+int32_t b2a_conv1d_fused_fits(int32_t span, int32_t N, int32_t C, int32_t wplanes, int32_t planes);
 /* tiling of the calling host thread's last successful b2a_conv1d_fused launch: out[0] = problems, out[1] = grid (CTAs),
  * out[2 + 2 i], out[3 + 2 i] = N tile and K split of problem i in the caller's order (i < 4, unused slots zero).  Host-side only. */
 int32_t b2a_conv1d_fused_last_config(int32_t* out10);

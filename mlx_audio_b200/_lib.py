@@ -99,6 +99,7 @@ PROTOTYPES = {
     "b2a_conv1d_fused_debug": (i32, [c_f]),
     "b2a_conv1d_fused_last_config": (i32, [C.POINTER(i32)]),
     "b2a_conv1d_fused": (i32, [C.POINTER(ConvFParams), i32, i32, i32, c_f, i64, C.c_void_p]),
+    "b2a_conv1d_fused_fits": (i32, [i32, i32, i32, i32, i32]),
     "b2a_copy2d": (i32, [c_f, i64, c_f, i64, i64, i32, C.c_void_p]),
     "b2a_gather_rows": (i32, [c_f, i64, c_f, c_f, i64, i64, i32, i64, c_f, i64, i64, C.c_void_p]),
     "b2a_durations_to_index": (i32, [c_f, c_f, i32, f32, c_f, c_f, i64, c_f, C.c_void_p]),

@@ -87,6 +87,8 @@ struct FParams {
                                                // results are then garbage -- timing only
   FProb pr[MAXG];
 };
+// dynamic shared memory a launch may take: the kernel keeps a static shared copy of FParams beside it
+constexpr size_t DYN_SMEM_MAX = (size_t)227 * 1024 - ((sizeof(FParams) + 1023) & ~(size_t)1023);
 
 struct TileRef { int g, b, mt, nt, ks; };
 
@@ -735,6 +737,30 @@ int get_enc() {
   return 0;
 }
 
+// N tile: the widest divisor of N (multiple of 32, <= 128) -- in polyphase mode also a divisor of C so that a tile stays inside one phase
+int n_tile(int N, int C) {
+  for (int c = 128; c >= 32; c -= 32) if (N % c == 0 && C % c == 0) return c;
+  return 0;
+}
+int a_rows(int span) { return (TM + span + 7) / 8 * 8; }     // rows of one K chunk's A tile: 128 output rows + the taps' span, to 8
+int acc_tile_ld(int bn) { return bn + 8; }                    // 8 mod 32 words: the accumulator fragment stores of a quarter-warp hit distinct banks
+// GEMM rows: the output rows, or in polyphase mode every row m whose phases m * s + r - crop reach an output row below Lout.  Rows past
+// L + taps - 1 read only the zero padding, so output rows past the scatter (output padding wider than the crop) get the epilogue alone.
+int gemm_rows(const b2a_convf_t& q) {
+  if (q.up_stride <= 0) return q.Lout;
+  const int tail = cdiv(q.Lout + q.up_crop, q.up_stride);
+  return q.L + q.taps - 1 > tail ? q.L + q.taps - 1 : tail;
+}
+// Weight stages (at most 8) that fit beside the two A buffers, the output tile and the fixed regions; *smem: the launch's dynamic
+// shared memory with that many stages.  A launch needs two.
+int weight_stages(int a_plane, int planes, int acc_ld, int w_stage, size_t* smem) {
+  const size_t fixed = (size_t)2 * a_plane * planes + (size_t)TM * acc_ld * 4 + SACC + CTAB + 1024 /*align*/ + 512 /*barriers*/;
+  int wst = fixed < DYN_SMEM_MAX ? (int)((DYN_SMEM_MAX - fixed) / w_stage) : 0;
+  if (wst > 8) wst = 8;
+  if (smem) *smem = fixed + (size_t)wst * w_stage;
+  return wst;
+}
+
 int make_wmap(CUtensorMap* m, const void* base, uint64_t cin_pad, uint64_t rows, uint32_t bn, int f16) {
   cuuint64_t gd[2] = {cin_pad, rows};
   cuuint64_t gs[1] = {cin_pad * 2};
@@ -755,6 +781,13 @@ extern "C" int32_t b2a_conv1d_fused_last_config(int32_t* out10) {
   B2A_CHECK_ARG(out10, "null pointer");
   for (int i = 0; i < 2 + 2 * MAXG; i++) out10[i] = g_last_cfg[i];
   return B2A_OK;
+}
+
+/* whether one problem of this geometry fits a launch's shared memory (see include/b200audio.h) */
+extern "C" int32_t b2a_conv1d_fused_fits(int32_t span, int32_t N, int32_t C, int32_t wplanes, int32_t planes) {
+  if (span < 0 || span > 64 || N <= 0 || C <= 0 || N % C || (wplanes != 1 && wplanes != 2) || (planes != 1 && planes != 2)) return 0;
+  const int bn = n_tile(N, C);
+  return bn && weight_stages(a_rows(span) * 128, planes, acc_tile_ld(bn), bn * 128 * wplanes, nullptr) >= 2;
 }
 
 extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream) {
@@ -781,11 +814,9 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
   for (int gi = 0; gi < n; gi++) {                         // output tiles of the whole launch before any split (same tile rule as below)
     const b2a_convf_t& q = pr[gi];
     if (q.N <= 0 || q.N % 32) continue;                    // rejected by the argument checks below
-    const int C_ = q.up_stride > 0 ? q.N / q.up_stride : q.N;
-    int bn = 32;
-    for (int c = 128; c >= 32; c -= 32) if (q.N % c == 0 && C_ % c == 0) { bn = c; break; }
-    const int mrows = q.up_stride > 0 ? q.L + q.taps - 1 : q.Lout;
-    sum_base += (int64_t)cdiv(mrows, TM) * (q.N / bn) * q.B;
+    const int bn = n_tile(q.N, q.up_stride > 0 ? q.N / q.up_stride : q.N);
+    if (!bn) continue;
+    sum_base += (int64_t)cdiv(gemm_rows(q), TM) * (q.N / bn) * q.B;
   }
   for (int gi = 0; gi < n; gi++) {
     const b2a_convf_t& q = pr[order[gi]];
@@ -807,14 +838,11 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
     int smin = q.shifts[0], smax = q.shifts[0];
     for (int i = 0; i < q.taps; i++) { P.shift[i] = q.shifts[i]; smin = q.shifts[i] < smin ? q.shifts[i] : smin; smax = q.shifts[i] > smax ? q.shifts[i] : smax; }
     if (smax - smin > 64) { b2a_set_error("b2a_conv1d_fused: taps span %d rows (> 64)", smax - smin); return B2A_E_UNSUPPORTED; }
-    P.shift_min = smin; P.R = (TM + (smax - smin) + 7) / 8 * 8;
+    P.shift_min = smin; P.R = a_rows(smax - smin);
     P.up_s = q.up_stride; P.up_crop = q.up_crop; P.C = q.up_stride ? q.N / q.up_stride : q.N;
-    P.Lout = q.Lout; P.Mrows = q.up_stride ? q.L + q.taps - 1 : q.Lout;
+    P.Lout = q.Lout; P.Mrows = gemm_rows(q);
     P.ntm = cdiv(P.Mrows, TM);
-    // N tile: the widest divisor of N (multiple of 32, <= 128) -- in polyphase mode also a divisor of C so that a tile stays inside one phase
-    int bn = 0;
-    for (int c = 128; c >= 32; c -= 32) if (q.N % c == 0 && P.C % c == 0) { bn = c; break; }
-    P.BN = bn; P.ntn = q.N / bn;
+    P.BN = n_tile(q.N, P.C); P.ntn = q.N / P.BN;
     base_tiles = (int64_t)P.ntm * P.ntn * q.B;
     // split K across CTAs when the whole launch cannot give every SM a tile (every problem of a group by the same rule: the decoder
     // blocks -- a k=3 conv over 390 rows grouped with its 1x1 shortcut -- are 48 tiles with 54 tap steps each)
@@ -861,14 +889,11 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
   }
   p.a_plane = maxR * 128;
   p.w_stage = maxWst;
-  p.acc_ld = maxBN + 8;                                  // 8 mod 32 words: the accumulator fragment stores of a quarter-warp hit distinct banks
-  const size_t DYN_SMEM_MAX = (size_t)227 * 1024 - ((sizeof(FParams) + 1023) & ~(size_t)1023);   // the kernel keeps a static shared copy of FParams
-  const size_t fixed = (size_t)2 * p.a_plane * planes + (size_t)TM * p.acc_ld * 4 + SACC + CTAB + 1024 /*align*/ + 512 /*barriers*/;
-  int wst = (int)((DYN_SMEM_MAX - fixed) / p.w_stage);   // the kernel keeps a static shared copy of FParams
-  if (wst > 8) wst = 8;
+  p.acc_ld = acc_tile_ld(maxBN);
+  size_t smem = 0;
+  const int wst = weight_stages(p.a_plane, planes, p.acc_ld, p.w_stage, &smem);
   if (wst < 2) { b2a_set_error("b2a_conv1d_fused: shared memory cannot hold two weight stages (R %d, BN %d)", maxR, maxBN); return B2A_E_UNSUPPORTED; }
   p.wst = wst;
-  const size_t smem = fixed + (size_t)wst * p.w_stage;
 
   CUtensorMap mw[MAXG], ml[MAXG];
   for (int gi = 0; gi < MAXG; gi++) {

@@ -393,7 +393,9 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
   p.f16 = f16 ? 1 : 0;
   p.wplanes = w_lo ? 2 : 1;
   p.up_s = up_stride; p.up_crop = up_crop; p.C = up_stride ? Cout / up_stride : Cout;
-  p.Mrows = up_stride ? L + taps - 1 : Lout;
+  // GEMM rows: in polyphase mode every row m whose phases m * up_stride + r - up_crop reach an output row below Lout.  Rows past
+  // L + taps - 1 read only the zero padding (TMA fills rows past L with zeros), so output rows past the scatter get the epilogue alone.
+  p.Mrows = up_stride ? (L + taps - 1 > cdiv(Lout + up_crop, up_stride) ? L + taps - 1 : cdiv(Lout + up_crop, up_stride)) : Lout;
   p.B = B; p.L = L; p.Lout = Lout; p.Cout = Cout; p.cin_pad = cin_pad; p.taps = taps; p.planes = a_lo ? 2 : 1;
   // N tile = the widest divisor of Cout that is a multiple of 32 (the epilogue's chunk) and <= 128 (the register accumulator).  96 matters:
   // the Qwen3 vocoder's 96-, 192- and 384-channel blocks would otherwise run as 32-/64-wide tiles and re-read A three times.

@@ -362,7 +362,7 @@ def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, 
         r, r_bs, r_ld = res.data_ptr(), (res.stride(0) if res.shape[0] == B else 0), res.stride(1)
     ws, slots = None, 0
     if stats and TC_STATS[0]:          # InstanceNorm partials of the output straight from the epilogue (persistent kernel only)
-        mrows = (L + taps - 1) if up_stride else lout
+        mrows = max(L + taps - 1, -(-(lout + pad_left) // up_stride)) if up_stride else lout      # b2a_conv1d_tc's GEMM rows
         slots = -(-mrows // 128) * 4 * max(1, up_stride)
         ws = torch.empty(B, slots, cw.cout, 2, device=hi.device, dtype=torch.float64)
     _call("conv_tc", _lib.lib().b2a_conv1d_tc, 1, hi.data_ptr(), _p(lo), int(cw.f16), B, L, cw.cin_pad, w_tc.data_ptr(), _p(w_lo), taps, shifts, n_total, lout,
@@ -464,7 +464,8 @@ def _al16(t: Optional[torch.Tensor]) -> bool:
 
 def fused_eligible(x, cw: "ConvW", stride: int = 1, dilation: int = 1, transpose: bool = False, pad_mode: int = 0, out=None, res=None) -> bool:
     """Dense layers the fused kernel takes: tensor-core weights, stride 1 (or a polyphase transposed conv), taps spanning <= 64 rows,
-    16-byte aligned fp32 rows."""
+    16-byte aligned fp32 rows, and room in shared memory for two weight stages (split fp32 weights at BN 128 in "x2" mode: a span of
+    at most 24 rows; b2a_conv1d_fused_fits decides)."""
     if not FUSED[0] or TC_MODE[0] == "off" or cw.w_tc is None or pad_mode != 0 or cw.cout % 32 != 0 or cw.groups != 1 or isinstance(x, Planes):
         return False
     if x.dtype != torch.float32 or x.dim() != 3 or x.stride(2) != 1 or x.stride(1) % 4 or x.stride(0) % 4 or x.data_ptr() % 16:
@@ -472,8 +473,14 @@ def fused_eligible(x, cw: "ConvW", stride: int = 1, dilation: int = 1, transpose
     if x.stride(1) < -(-x.shape[2] // 4) * 4 or not _al16(out) or not _al16(res):
         return False
     if transpose:
-        return dilation == 1 and cw.K % stride == 0 and cw.K // stride <= 32 and cw.cin * (cw.K // stride) >= TC_MIN_K
-    return stride == 1 and cw.K <= 32 and (cw.K - 1) * dilation <= 64 and cw.cin * cw.K >= TC_MIN_K
+        if not (dilation == 1 and cw.K % stride == 0 and cw.K // stride <= 32 and cw.cin * (cw.K // stride) >= TC_MIN_K):
+            return False
+        span, n_total = cw.K // stride - 1, stride * cw.cout
+    else:
+        if not (stride == 1 and cw.K <= 32 and cw.cin * cw.K >= TC_MIN_K):
+            return False
+        span, n_total = (cw.K - 1) * dilation, cw.cout
+    return bool(_lib.lib().b2a_conv1d_fused_fits(span, n_total, cw.cout, 1 if cw.w_tc_lo is None else 2, 2 if TC_MODE[0] == "x2" else 1))
 
 
 class FusedProblem:
