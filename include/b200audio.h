@@ -630,6 +630,33 @@ int32_t b2a_encodec_normalize(const float* x, int64_t x_bs, int64_t x_ld, int32_
 int32_t b2a_encodec_ola(const float* frames, int32_t N, int32_t B, int32_t L, int32_t C, const float* scale, int32_t stride, int32_t Tout,
                         float* out, void* stream);
 
+/* ---- Soprano TTS (soprano.cu; tts/models/soprano/soprano.py, decoder.py) ------------------------------------------------------
+ * mlx-lm's make_sampler(temperature, top_p) (lm/sample_utils.py:11-70) as soprano.py:336-346 applies it, to RAW logits [B, V] (row
+ * stride logits_bs), one CTA per row:
+ *   temperature == 0: argmax, the first index on ties (soprano.py:343-344);
+ *   0 < top_p < 1: apply_top_p (sample_utils.py:206-238) on the raw logits: a token is kept iff the inclusive cumulative sum of
+ *     exp(logit) in ascending order (ties: lower index first) exceeds 1 - top_p.  exp is fp32 (an overflow to inf keeps every token from
+ *     that rank up), the sums are float64 in a fixed order.  When nothing is kept (every logit -inf) the token is 0, MLX's categorical
+ *     of an all -inf row;
+ *   then categorical_sampling (:279): logits * float32(1 / temperature), drawn by the inverse CDF in index order of their softmax with
+ *     u[b * u_bs + step] in [0, 1), step = *step_dev (0 when NULL).
+ * Writes out[b] and hist[b * hist_bs + step] (hist may be NULL); a row whose token is stop0 or stop1 gets finished[b] = 1, and a row
+ * with finished[b] set writes nothing (finished may be NULL).  A row's result does not depend on B.  Any V >= 1; rows of at most
+ * 36 864 logits are staged in shared memory, longer ones are read from global memory on each of the 8 radix passes. */
+int32_t b2a_lm_sample_mlx(const float* logits, int64_t logits_bs, int32_t B, int32_t V, float temperature, double top_p, const float* u,
+                          int64_t u_bs, const int32_t* step_dev, int64_t* out, int64_t* hist, int64_t hist_bs, uint8_t* finished,
+                          int32_t stop0, int32_t stop1, void* stream);
+/* SopranoDecoder's up-sampling (decoder.py:102-112 with interpolate.py:61-117, mode "linear", align_corners=True): x [B, L, H] (strides
+ * x_bs, x_ld) -> Lo = up (L - 1) + 1 rows, row i = x[lo] (1 - f) + x[hi] f in fp32 with pos = float(i) * float((L - 1) / (Lo - 1)),
+ * lo = floor(pos), hi = min(lo + 1, L - 1), f = pos - lo (for up = 4: 0, .25, .5, .75); L = 1 broadcasts the row.  Output fp32 y (strides
+ * y_bs, y_ld) or the bf16 hi / lo planes [B, Lo, cpad] of the next tensor-core conv (lo may be NULL; channels >= H are 0). */
+int32_t b2a_soprano_upsample(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t H, int32_t up, float* y, int64_t y_bs,
+                             int64_t y_ld, void* hi, void* lo, int32_t cpad, void* stream);
+/* dst[b * dst_bs + r * dst_ld + c] = src[b * src_bs + c] for c < H with r = *idx_dev + add: one hidden row per batch row stored at a
+ * device-resident step index (rows outside [0, cap) are skipped). */
+int32_t b2a_soprano_store_rows(const float* src, int64_t src_bs, int32_t B, int32_t H, float* dst, int64_t dst_bs, int64_t dst_ld,
+                               const int32_t* idx_dev, int32_t add, int32_t cap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

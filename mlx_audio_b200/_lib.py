@@ -172,6 +172,9 @@ PROTOTYPES = {
     "b2a_encodec_gn_coeffs": (i32, [c_f, i64, i64, i32, i32, i32, c_f, c_f, f32, c_f, c_f, c_f, C.c_void_p]),
     "b2a_encodec_normalize": (i32, [c_f, i64, i64, i32, i32, i32, c_f, i64, c_f, c_f, C.c_void_p]),
     "b2a_encodec_ola": (i32, [c_f, i32, i32, i32, i32, c_f, i32, i32, c_f, C.c_void_p]),
+    "b2a_lm_sample_mlx": (i32, [c_f, i64, i32, i32, f32, C.c_double, c_f, i64, c_f, c_f, c_f, i64, c_f, i32, i32, C.c_void_p]),
+    "b2a_soprano_upsample": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, i64, i64, c_f, c_f, i32, C.c_void_p]),
+    "b2a_soprano_store_rows": (i32, [c_f, i64, i32, i32, c_f, i64, i64, c_f, i32, i32, C.c_void_p]),
 }
 
 E_INVALID, E_CUDA, E_UNSUPPORTED = -1, -2, -3

@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200audio.so")
-SOURCES = ["api.cu", "conv.cu", "norm.cu", "attn.cu", "lstm.cu", "dsp.cu", "codec.cu", "gemm_tc.cu", "sampler.cu", "lm.cu", "attn_tc.cu", "conv_fused.cu", "stream.cu", "speaker.cu", "attn_prefill.cu", "mimi_stream.cu", "albert.cu", "dac.cu", "bigvgan.cu", "vocos.cu", "encodec.cu"]
+SOURCES = ["api.cu", "conv.cu", "norm.cu", "attn.cu", "lstm.cu", "dsp.cu", "codec.cu", "gemm_tc.cu", "sampler.cu", "lm.cu", "attn_tc.cu", "conv_fused.cu", "stream.cu", "speaker.cu", "attn_prefill.cu", "mimi_stream.cu", "albert.cu", "dac.cu", "bigvgan.cu", "vocos.cu", "encodec.cu", "soprano.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas=-v"]
 

@@ -229,15 +229,17 @@ class VocosBackbone:
         return ops.linear(c.contiguous(), self._W["ada"])          # [B, (num_layers + 1) * 2 dim]: (scale | shift) per norm
 
     def forward(self, x, bandwidth_id=None, planes_for: Optional[ops.ConvW] = None):
-        """-> [B, T, dim] fp32, or the bf16 planes of ``planes_for`` (the head linear) when that layer runs on the tensor cores."""
+        """x [B, T, C] / [B, C, T] / [T, C], or the bf16 ``Planes`` of the embed conv -> [B, T, dim] fp32, or the bf16 planes of
+        ``planes_for`` (the head linear) when that layer runs on the tensor cores."""
         self._ensure_weights()
         W, d = self._W, self.dim
-        x = torch.as_tensor(x).to(device=self.device, dtype=torch.float32)
-        if x.dim() == 2:
-            x = x[None]
-        if x.shape[-1] != self.input_channels:                      # vocos.py:259-261, ambiguous when T == C
-            x = x.transpose(1, 2)
-        x = x.contiguous()
+        if not isinstance(x, ops.Planes):                            # Planes: the embed conv's operand, already split by its producer
+            x = torch.as_tensor(x).to(device=self.device, dtype=torch.float32)
+            if x.dim() == 2:
+                x = x[None]
+            if x.shape[-1] != self.input_channels:                  # vocos.py:259-261, ambiguous when T == C
+                x = x.transpose(1, 2)
+            x = x.contiguous()
         B, T, _ = x.shape
         ada = self._cond(bandwidth_id, B)
         a = lambda i: None if ada is None else ada[:, 2 * d * i: 2 * d * (i + 1)]

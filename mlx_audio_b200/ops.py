@@ -1590,3 +1590,61 @@ def encodec_ola(frames: torch.Tensor, B: int, scale: Optional[torch.Tensor], str
     out = torch.empty(B, t_out, Cc, device=frames.device, dtype=torch.float32)
     _call("other", _lib.lib().b2a_encodec_ola, 1, frames.data_ptr(), NB // B, B, L, Cc, _p(scale), stride, t_out, out.data_ptr(), _stream())
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------- Soprano
+def lm_sample_mlx(logits: torch.Tensor, *, temperature: float, top_p: float, u: Optional[torch.Tensor] = None,
+                  step_dev: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, hist: Optional[torch.Tensor] = None,
+                  finished: Optional[torch.Tensor] = None, stop_ids=()) -> torch.Tensor:
+    """mlx-lm's ``make_sampler(temperature, top_p)`` on raw logits [B, V] (row stride free, unit column stride) -> int64 tokens [B]
+    (b2a_lm_sample_mlx).  ``u`` float32 [B, n]: the draw of row b at step s is u[b, s], s = ``step_dev`` (int32 [1]) or 0.  ``hist`` int64
+    [B, n] receives the token at column s.  ``finished`` uint8 [B]: rows set there write nothing; a row drawing one of ``stop_ids`` (at most
+    two) is set."""
+    B, V = logits.shape
+    if logits.dtype != torch.float32 or not logits.is_cuda or logits.stride(1) != 1:
+        raise ValueError("lm_sample_mlx: logits must be a CUDA float32 [B, V] tensor with unit column stride")
+    if temperature > 0 and (u is None or u.dtype != torch.float32 or u.dim() != 2 or u.shape[0] != B or u.stride(1) != 1):
+        raise ValueError("lm_sample_mlx: temperature > 0 needs float32 uniforms u [B, steps]")
+    stops = [int(s) for s in stop_ids if s is not None]
+    if len(stops) > 2:
+        raise ValueError("lm_sample_mlx: at most two stop ids")
+    stops += [-1] * (2 - len(stops))
+    if out is None:
+        out = torch.empty(B, device=logits.device, dtype=torch.int64)
+    assert out.dtype == torch.int64 and out.is_contiguous() and out.numel() == B
+    assert step_dev is None or (step_dev.dtype == torch.int32 and step_dev.is_cuda)
+    assert hist is None or (hist.dtype == torch.int64 and hist.dim() == 2 and hist.stride(1) == 1 and hist.shape[0] == B)
+    assert finished is None or (finished.dtype == torch.uint8 and finished.is_contiguous() and finished.numel() == B)
+    _call("sampler", _lib.lib().b2a_lm_sample_mlx, 1, logits.data_ptr(), logits.stride(0), B, V, float(temperature), float(top_p), _p(u),
+          0 if u is None else u.stride(0), _p(step_dev), out.data_ptr(), _p(hist), 0 if hist is None else hist.stride(0), _p(finished),
+          stops[0], stops[1], _stream())
+    return out
+
+
+def soprano_upsample(x: torch.Tensor, up: int, *, planes_for: Optional[ConvW] = None):
+    """SopranoDecoder's align-corners linear up-sampling (decoder.py:102-112): x [B, L, H] -> fp32 [B, up (L - 1) + 1, H], or with
+    ``planes_for`` the bf16 ``Planes`` of that tensor-core conv (``conv1d(planes, planes_for, ...)`` takes them with no prologue)."""
+    _chk3(x, "soprano_upsample x")
+    B, L, H = x.shape
+    Lo = up * (L - 1) + 1
+    if planes_for is not None:
+        if planes_for.cin != H or planes_for.w_tc is None or planes_for.f16:
+            raise ValueError("soprano_upsample: planes_for must be a bf16 tensor-core conv taking the hidden width")
+        out = _new_planes(B, Lo, planes_for.cin_pad, x.device)
+        out.C = H
+        _call("other", _lib.lib().b2a_soprano_upsample, 1, x.data_ptr(), x.stride(0), x.stride(1), B, L, H, up, None, 0, 0,
+              out.hi.data_ptr(), _p(out.lo), planes_for.cin_pad, _stream())
+        return out
+    out = torch.empty(B, Lo, H, device=x.device, dtype=torch.float32)
+    _call("other", _lib.lib().b2a_soprano_upsample, 1, x.data_ptr(), x.stride(0), x.stride(1), B, L, H, up, out.data_ptr(), out.stride(0),
+          out.stride(1), None, None, 0, _stream())
+    return out
+
+
+def store_rows_at(src: torch.Tensor, dst: torch.Tensor, idx_dev: torch.Tensor, add: int = 0) -> None:
+    """dst[b, idx_dev[0] + add, :] = src[b, :] for src [B, H] and dst [B, T, H] float32 (rows outside [0, T) are skipped)."""
+    B, H = src.shape
+    assert src.dtype == dst.dtype == torch.float32 and src.stride(1) == 1 and dst.stride(2) == 1 and dst.shape[0] == B and dst.shape[2] == H
+    assert idx_dev.dtype == torch.int32 and idx_dev.is_cuda
+    _call("other", _lib.lib().b2a_soprano_store_rows, 1, src.data_ptr(), src.stride(0), B, H, dst.data_ptr(), dst.stride(0), dst.stride(1),
+          idx_dev.data_ptr(), int(add), dst.shape[1], _stream())

@@ -732,3 +732,37 @@ def encodec_weights(config: dict, seed=15) -> dict:
             gain = 1 / math.sqrt(2) if (".block.3." in name or ".shortcut." in name) else 1.0
             P[name] = gain / math.sqrt(shape[1] * shape[2]) * torch.randn(*shape, generator=g)
     return P
+
+
+# reference test configuration of Soprano's LM (tts/tests/test_models.py TestSoprano), 12 layers
+SOPRANO_LM = {"hidden_size": 512, "num_hidden_layers": 12, "num_attention_heads": 8, "num_key_value_heads": 4, "intermediate_size": 1024,
+              "vocab_size": 32000, "head_dim": 64, "rms_norm_eps": 1e-5, "rope_theta": 10000.0, "max_position_embeddings": 4096,
+              "tie_word_embeddings": False, "model_type": "qwen3"}
+
+
+def soprano_weights(model, seed=21, logit_std=4.0) -> dict:
+    """Sanitized parameters of a ``tts.models.soprano.Model``: the Qwen3 LM (``language_model.*``, fan-in scaled bf16-exact values, a head
+    whose logits have a spread of about ``logit_std`` so that top-p filtering bites) and the decoder (``decoder.decoder.*``,
+    ``decoder.head.*``)."""
+    c = model.config
+    g = _Gen(seed)
+    gen = g.g
+    H, I, hd, hq, hk = c.hidden_size, c.intermediate_size, c.head_dim, c.num_attention_heads, c.num_key_value_heads
+    for i in range(c.num_hidden_layers):
+        L = f"language_model.layers.{i}"
+        _fan(g, L + ".self_attn.q_proj.weight", hq * hd, H, fan_in=H)
+        _fan(g, L + ".self_attn.k_proj.weight", hk * hd, H, fan_in=H)
+        _fan(g, L + ".self_attn.v_proj.weight", hk * hd, H, fan_in=H)
+        _fan(g, L + ".self_attn.o_proj.weight", H, hq * hd, fan_in=4 * hq * hd)
+        for n, d in ((".self_attn.q_norm.weight", hd), (".self_attn.k_norm.weight", hd), (".input_layernorm.weight", H),
+                     (".post_attention_layernorm.weight", H)):
+            g.P[L + n] = _bf16(1.0 + 0.1 * torch.randn(d, generator=gen))
+        _fan(g, L + ".mlp.gate_proj.weight", I, H, fan_in=H)
+        _fan(g, L + ".mlp.up_proj.weight", I, H, fan_in=H)
+        _fan(g, L + ".mlp.down_proj.weight", H, I, fan_in=4 * I)
+    g.P["language_model.norm.weight"] = _bf16(1.0 + 0.1 * torch.randn(H, generator=gen))
+    g.normal("language_model.embed_tokens.weight", c.vocab_size, H, std=1.0)
+    _fan(g, "language_model.lm_head.weight", c.vocab_size, H, fan_in=H / logit_std ** 2)
+    g.P.update(vocos_backbone_weights(model.decoder.decoder, seed=seed + 1, prefix="decoder.decoder."))
+    g.P.update(vocos_head_weights(model.decoder.head, seed=seed + 2, prefix="decoder.head."))
+    return g.P

@@ -15,7 +15,7 @@ import torch
 
 from .dsp import STR_TO_WINDOW_FN, ISTFTCache, bartlett, blackman, hamming, hanning, istft, mel_filters, stft  # noqa: F401 (utils.py:31-40 re-exports)
 
-MODEL_REMAPPING = {"tts": {"kokoro": "kokoro", "qwen3_tts": "qwen3_tts"}, "stt": {"whisper": "whisper"}}
+MODEL_REMAPPING = {"tts": {"kokoro": "kokoro", "qwen3_tts": "qwen3_tts", "soprano": "soprano"}, "stt": {"whisper": "whisper"}}
 
 
 def get_model_path(path_or_repo: str, **_) -> Path:
@@ -33,13 +33,21 @@ def load_config(model_path: Path) -> dict:
         return json.load(f)
 
 
-def get_model_class(model_type: str, category: str):
-    """utils.py:259-318: import <category>.models.<model_type> and return the module exposing Model / ModelConfig."""
-    model_type = MODEL_REMAPPING.get(category, {}).get(model_type, model_type)
+def get_model_class(model_type: str, category: str, model_name=None):
+    """utils.py:259-318: import <category>.models.<model_type> and return the module exposing Model / ModelConfig.  When the type does
+    not resolve (a Soprano checkpoint says ``model_type: "qwen3"``), a part of the directory name ``model_name`` (its "-" separated
+    pieces) that names a model of the category is used instead, as the reference's name hint does."""
+    remap = MODEL_REMAPPING.get(category, {})
+    mapped = remap.get(model_type, model_type)
     try:
-        return importlib.import_module(f"mlx_audio_b200.{category}.models.{model_type}")
+        return importlib.import_module(f"mlx_audio_b200.{category}.models.{mapped}")
     except ImportError as e:
-        raise ValueError(f"Model type {model_type} not supported for {category} on the H100 path") from e
+        if e.name != f"mlx_audio_b200.{category}.models.{mapped}":
+            raise
+        hint = next((remap[p] for p in (model_name or []) if p in remap), None)
+        if hint is None:
+            raise ValueError(f"Model type {model_type} not supported for {category} on the H100 path") from e
+        return importlib.import_module(f"mlx_audio_b200.{category}.models.{hint}")
 
 
 def load_weights(model_path: Path) -> dict:
@@ -64,8 +72,10 @@ def base_load_model(model_path, category: str, lazy: bool = False, strict: bool 
         mt = next((p for p in parts if p in known), None)
     if mt is None:
         raise ValueError(f"Could not determine model_type for {model_path}")
-    mod = get_model_class(mt, category)
+    mod = get_model_class(mt, category, path.name.lower().replace("_", "-").split("-"))
     cfg_cls = getattr(mod, "ModelConfig", None)
+    if cfg_cls is not None and "model_path" in getattr(cfg_cls, "__dataclass_fields__", {}):
+        config = {**config, "model_path": str(model_path)}              # utils.py:365 (Soprano picks its decoder from it)
     cfg = cfg_cls.from_dict(config) if cfg_cls is not None and hasattr(cfg_cls, "from_dict") else config
     model = mod.Model(cfg, device=device)
     weights = load_weights(path)
