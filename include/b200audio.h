@@ -116,9 +116,8 @@ int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16, int32_t B
                       int32_t taps, const int32_t* shifts_host, int32_t Cout, int32_t Lout, const float* bias,
                       int32_t post_act, float post_p0, const float* cscale, int64_t cscale_bs, const float* res,
                       int64_t res_bs, int64_t res_ld, int32_t res_div, float out_scale, int32_t accumulate, float* y,
-                      int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop, double* stats_ws,
-                      int32_t stats_slots, void* emit_hi, void* emit_lo, int64_t emit_ld, void* attn_ws, int32_t attn_heads,
-                      float attn_scale, void* stream);
+                      int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop, void* emit_hi, void* emit_lo,
+                      int64_t emit_ld, void* attn_ws, int32_t attn_heads, float attn_scale, void* stream);
 /* b2a_conv1d_tc also writes its consumer's A operand from the epilogue (up_stride == 0 only; at most one of the two):
  *   emit_hi != NULL: bf16 planes bf16(y), bf16(y - hi) [B, Lout, emit_ld] (lo == NULL: hi only) -- what b2a_prep_bf16 makes of y;
  *   attn_ws != NULL: y is a fused [q | k | v] projection (Cout = 3 * 64 * attn_heads) and the epilogue fills b2a_attention_tc's
@@ -180,11 +179,6 @@ int32_t b2a_durations_to_index(const float* dur_f, const int64_t* dur_i, int32_t
 int64_t b2a_adain_ws_bytes(int32_t B, int32_t L, int32_t C);
 int32_t b2a_adain_coeffs(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t C,
                          const float* gb, float eps, float* scale, float* shift, void* ws, void* stream);
-/* Same coefficients from partial sums a producer already wrote: partials [B][nslots][C][2] float64 (sum, sum of squares per row group).
- * b2a_conv1d_tc(stats_ws != NULL) emits them from its epilogue -- one slot per 32 output rows (times the up-sampling factor in
- * transposed mode; stats_slots = ceil(Mrows/128)*4*max(1, up_stride)) -- so AdaIN-conv chains skip the statistics pass over HBM. */
-int32_t b2a_adain_coeffs_from_partials(const double* partials, int32_t nslots, int32_t B, int32_t L, int32_t C, const float* gb,
-                                       float eps, float* scale, float* shift, void* stream);
 /* (sum, sumsq) over L of every channel of x [B, L, C], ADDED to n_dst (1..4) binned accumulators laid out [B][.][2][4] int64; dst[i] points
  * at the first channel's bins, dst_bs[i] int64 elements separate batches.  This is the statistics format b2a_conv1d_fused consumes (pre_mode 2)
  * and produces (stats_out); the stand-alone kernel covers tensors no fused conv produced (LSTM outputs, concatenated side channels). */
@@ -389,14 +383,6 @@ int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, const float
                          int64_t c_ss, float* out, int64_t o_bs, int64_t o_ss, int32_t B, int32_t S, int32_t Hq, int32_t Hkv,
                          int32_t D, float scale, const int32_t* base_dev, int32_t base_host, const int32_t* kv_start,
                          int32_t max_k, const int32_t* base_rows, const int32_t* slot, void* stream);
-/* Single-token decode (S = 1, GQA group of 2): b2a_qknorm_rope_cache + b2a_attn_decode in one launch, one CTA per (kv head, batch)
- * -- each cache row is read once for both query heads of the group.  qkv [B, (Hq+2Hkv) D]; out [B, Hq*D]; pos3 [3,B] or NULL.
- * base_rows / slot as in b2a_qknorm_rope_cache (a negative base writes nothing and gives a zero output). */
-int32_t b2a_attn_decode_fused(const float* qkv, int64_t qkv_bs, int32_t B, int32_t Hq, int32_t Hkv, int32_t D, const float* q_norm_w,
-                              const float* k_norm_w, float eps, const int32_t* pos3, const int32_t* base_dev, int32_t base_host,
-                              int32_t sec_h, int32_t sec_w, float theta, float* k_cache, float* v_cache, int64_t c_bs, int64_t c_ss,
-                              int32_t smax, float scale, const int32_t* kv_start, float* out, int64_t o_bs, const int32_t* base_rows,
-                              const int32_t* slot, void* stream);
 /* y[r, i] = silu(gate) * up (talker.py:319-321, speech_tokenizer.py:321-322) for the batched (prefill) path: x [rows, 2I] holds
  * (gate | up) halves, or interleaved (gate_0, up_0, gate_1, ...) pairs -- the row order b2a_gemv_bf16 mode 1 uses. */
 int32_t b2a_swiglu(const float* x, int64_t x_ld, int64_t rows, int32_t I, int32_t interleaved, float* y, int64_t y_ld, void* stream);

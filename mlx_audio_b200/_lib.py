@@ -93,7 +93,7 @@ PROTOTYPES = {
     "b2a_conv1d_cl_last_path": (i32, [C.POINTER(i32)]),
     "b2a_prep_bf16": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, i32, f32, c_f, c_f, c_f, c_f, i32, C.c_void_p]),
     "b2a_conv1d_tc": (i32, [c_f, c_f, i32, i32, i32, i32, c_f, c_f, i32, C.POINTER(i32), i32, i32, c_f, i32, f32, c_f, i64, c_f, i64, i64, i32, f32, i32,
-                            c_f, i64, i64, i32, i32, c_f, i32, c_f, c_f, i64, c_f, i32, f32, C.c_void_p]),
+                            c_f, i64, i64, i32, i32, c_f, c_f, i64, c_f, i32, f32, C.c_void_p]),
     "b2a_conv1d_tc_debug": (i32, [c_f]),
     "b2a_conv1d_tc_last_config": (i32, [C.POINTER(i32)]),
     "b2a_conv1d_fused_debug": (i32, [c_f]),
@@ -105,7 +105,6 @@ PROTOTYPES = {
     "b2a_durations_to_index": (i32, [c_f, c_f, i32, f32, c_f, c_f, i64, c_f, C.c_void_p]),
     "b2a_adain_ws_bytes": (i64, [i32, i32, i32]),
     "b2a_adain_coeffs": (i32, [c_f, i64, i64, i32, i32, i32, c_f, f32, c_f, c_f, c_f, C.c_void_p]),
-    "b2a_adain_coeffs_from_partials": (i32, [c_f, i32, i32, i32, i32, c_f, f32, c_f, c_f, C.c_void_p]),
     "b2a_channel_stats": (i32, [c_f, i64, i64, i32, i32, i32, C.POINTER(C.c_void_p), C.POINTER(i64), i32, C.c_void_p]),
     "b2a_coeffs_from_stats": (i32, [c_f, i32, i32, i32, c_f, f32, c_f, c_f, C.c_void_p]),
     "b2a_layernorm": (i32, [c_f, i64, c_f, i64, c_f, i64, i64, i32, c_f, c_f, c_f, f32, i32, i32, f32, c_f, c_f, i64, C.c_void_p]),
@@ -133,8 +132,6 @@ PROTOTYPES = {
                               C.c_void_p]),
     "b2a_attn_prefill": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, c_f, c_f,
                                C.c_void_p]),
-    "b2a_attn_decode_fused": (i32, [c_f, i64, i32, i32, i32, i32, c_f, c_f, f32, c_f, c_f, i32, i32, i32, f32, c_f, c_f, i64, i64, i32, f32,
-                                    c_f, c_f, i64, c_f, c_f, C.c_void_p]),
     "b2a_swiglu": (i32, [c_f, i64, i64, i32, i32, c_f, i64, C.c_void_p]),
     "b2a_embed_sum": (i32, [c_f, i64, i32, i32, i32, c_f, c_f, c_f, i64, i64, i32, c_f, c_f, i32, c_f, i64, c_f, c_f, c_f, C.c_void_p]),
     "b2a_incr_i32": (i32, [c_f, i32, C.c_void_p]),

@@ -79,8 +79,6 @@ struct FProb {
 
 struct FParams {
   int G, ntiles, planes, f16, wst, w_stage, a_plane, acc_ld;     // acc_ld: floats per row of the shared-memory output tile
-  int interleave;                              // 1: tile i belongs to problem i % G (equal tile counts, no split-K) -- see decode_tile
-  int ct_stride;                               // channels per problem in the coefficient table (CT_MAX, or CT_MAX / 4 when interleaved)
   unsigned long long* dbg;                     // optional [gridDim][32] globaltimer stamps (b2a_conv1d_fused_debug)
   int dbg_flags;                               // experiments (env B2A_FUSED_DBGFLAGS): 1 = converter skips the global loads, 2 = skips the smem stores,
                                                // 4 = skips fence.proxy.async, 16 = workers skip the conversion, 32 = skip the epilogue body;
@@ -92,17 +90,12 @@ constexpr size_t DYN_SMEM_MAX = (size_t)227 * 1024 - ((sizeof(FParams) + 1023) &
 
 struct TileRef { int g, b, mt, nt, ks; };
 
-// Tile order.  Contiguous: the tiles of the heaviest problem first.  Interleaved (groups whose problems have the same tile count, e.g. the
-// k = 3 / 7 / 11 resblocks of a generator stage): tile i belongs to problem i % G, so every CTA alternates between MMA-bound tiles (k = 11:
-// the workers wait for A buffers) and worker-bound ones (k = 3: the MMA warp waits for A chunks) and the two kinds overlap.
+// Tile order: the tiles of the heaviest problem first.
 __device__ __forceinline__ TileRef decode_tile(const FParams& p, int tile) {
-  int g = 0, local;
-  if (p.interleave) { g = tile % p.G; local = tile / p.G; }
-  else {
+  int g = 0;
 #pragma unroll
-    for (int i = 1; i < MAXG; i++) if (i < p.G && tile >= p.pr[i].tile_begin) g = i;
-    local = tile - p.pr[g].tile_begin;
-  }
+  for (int i = 1; i < MAXG; i++) if (i < p.G && tile >= p.pr[i].tile_begin) g = i;
+  int local = tile - p.pr[g].tile_begin;
   const FProb& P = p.pr[g];
   TileRef t;
   t.g = g;
@@ -299,7 +292,7 @@ __device__ __forceinline__ void mma_tile(const FParams& p, const FProb& P, const
 struct SmemLayout {
   int a_buf;
   uint8_t* wbase;
-  float *acct, *sacc, *ctab_all;             // ctab_all: [slots][2][ct_stride] scale | shift of the input transform
+  float *acct, *sacc, *ctab;                 // ctab: [2][CT_MAX] scale | shift of the input transform
   uint64_t *full, *empty, *tfull, *tempty, *a_full, *a_empty;   // a_full / a_empty: [2]
   int* flag_slot;
   __device__ __forceinline__ SmemLayout(uint8_t* smem, const FParams& p) {
@@ -307,8 +300,8 @@ struct SmemLayout {
     wbase = smem + (size_t)2 * a_buf;
     acct = reinterpret_cast<float*>(wbase + (size_t)p.wst * p.w_stage);
     sacc = acct + TM * p.acc_ld;
-    ctab_all = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sacc) + SACC);
-    full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ctab_all) + CTAB);
+    ctab = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sacc) + SACC);
+    full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ctab) + CTAB);
     empty = full + p.wst;
     tfull = empty + p.wst;
     tempty = tfull + 1;
@@ -428,7 +421,7 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
     set_regs<REG_WORK>();
     const SmemLayout sl(smem, p);
     const int a_buf = sl.a_buf;
-    float *const acct = sl.acct, *const sacc = sl.sacc, *const ctab_all = sl.ctab_all;
+    float *const acct = sl.acct, *const sacc = sl.sacc, *const ctab = sl.ctab;
     uint64_t *const a_full = sl.a_full, *const a_empty = sl.a_empty, *const tfull = sl.tfull, *const tempty = sl.tempty;
     int* const flag_slot = sl.flag_slot;
     // The first version of this kernel split the roles (8 converter + 8 epilogue warps).  Its profile on the Kokoro layers: the converter
@@ -447,7 +440,7 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
     const int quarter = ww & 3, sub = ww >> 2;       // quarter = 32-row group of the output tile; sub picks the 32-column chunk
     const int et = wt;
     uint32_t cg = 0;
-    int cur_key[MAXG] = {-1, -1, -1, -1};             // batch whose coefficients problem g's table holds (interleaved: one table per problem)
+    int cur_key = -1;                                // (problem, batch) whose coefficients the table holds
     unsigned long long w_aempty = 0, w_tfull = 0;
 
     auto convert_tile = [&](const int tile) {
@@ -480,25 +473,18 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
       const int R = P.R;
       // (scale, shift) of every input channel: computed once per (problem, batch) by the worker threads -- the float64 statistics
       // arithmetic costs ~150 double-precision operations per channel, far too much to repeat in every K chunk of every tile
-      const bool tabled = P.pre_mode != 0 && P.Cin <= p.ct_stride;
-      const int slot = p.interleave ? t.g : 0;
-      float* ctab = ctab_all + slot * 2 * p.ct_stride;
-      const int CTS = p.ct_stride;
+      const bool tabled = P.pre_mode != 0 && P.Cin <= CT_MAX;
       const int key = (t.g << 16) | t.b;
-      int have = cur_key[0];
-#pragma unroll
-      for (int i = 1; i < MAXG; i++) if (slot == i) have = cur_key[i];
-      if (tabled && key != have) {
+      if (tabled && key != cur_key) {
         bar_sync(3, NWORK * 32);                       // nobody still reads the previous table
         for (int c = wt; c < P.Cin; c += NWORK * 32) {
           float sc_ = P.in_scale, sh_ = 0.f;
           if (P.pre_mode == 1) { sc_ = __ldg(P.pre_scale + (int64_t)t.b * P.Cin + c) * P.in_scale; sh_ = __ldg(P.pre_shift + (int64_t)t.b * P.Cin + c); }
           else stats_coeffs(P, t.b, c, sc_, sh_);
-          ctab[c] = sc_; ctab[CTS + c] = sh_;
+          ctab[c] = sc_; ctab[CT_MAX + c] = sh_;
         }
         bar_sync(3, NWORK * 32);
-#pragma unroll
-        for (int i = 0; i < MAXG; i++) if (slot == i) cur_key[i] = key;
+        cur_key = key;
       }
       for (int kc = kc0; kc < kc1; kc++, cg++) {
         const uint32_t ab = cg & 1;
@@ -511,7 +497,7 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
           chok[q] = c < P.Cin;
           sc[q] = P.in_scale; sh[q] = 0.f; aa[q] = 1.f; bb[q] = 1.f;
           if (chok[q]) {
-            if (tabled) { sc[q] = ctab[c]; sh[q] = ctab[CTS + c]; }
+            if (tabled) { sc[q] = ctab[c]; sh[q] = ctab[CT_MAX + c]; }
             else if (P.pre_mode == 1) { sc[q] = __ldg(P.pre_scale + (int64_t)t.b * P.Cin + c) * P.in_scale; sh[q] = __ldg(P.pre_shift + (int64_t)t.b * P.Cin + c); }
             else if (P.pre_mode == 2) stats_coeffs(P, t.b, c, sc[q], sh[q]);
             if (P.pre_a) aa[q] = __ldg(P.pre_a + c);
@@ -793,12 +779,11 @@ extern "C" int32_t b2a_conv1d_fused_fits(int32_t span, int32_t N, int32_t C, int
 extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream) {
   B2A_CHECK_ARG(pr && n >= 1 && n <= MAXG && (planes == 1 || planes == 2), "1..4 problems, planes 1 or 2");
   if (get_enc() != 0) { b2a_set_error("b2a_conv1d_fused: cuTensorMapEncodeTiled entry point not found"); return B2A_E_CUDA; }
-  static int nsm = 0, pdl = -1, ksplit_on = -1;
+  static int nsm = 0, pdl = -1;
   if (!nsm) {
     int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
     if (nsm <= 0) nsm = 132;
     const char* e = getenv("B2A_FUSED_PDL"); pdl = (e && e[0] == '0') ? 0 : 1;
-    const char* k = getenv("B2A_FUSED_KSPLIT"); ksplit_on = (k && k[0] == '0') ? 0 : 1;
   }
   FParams p;
   p.G = n; p.planes = planes; p.f16 = f16 ? 1 : 0; p.dbg = g_fdbg;
@@ -809,8 +794,7 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
   for (int i = 0; i < n; i++) { order[i] = i; cost[i] = (double)pr[i].taps * pr[i].cin_pad; }
   for (int i = 0; i < n; i++) for (int j = i + 1; j < n; j++) if (cost[order[j]] > cost[order[i]]) { int t = order[i]; order[i] = order[j]; order[j] = t; }
   int maxR = 0, maxBN = 0, maxWst = 0, tiles_total = 0;
-  int64_t base_tiles = 0, sum_base = 0, cnt_used = 0, ws_used = 0, first_base = 0;
-  bool can_interleave = true;
+  int64_t base_tiles = 0, sum_base = 0, cnt_used = 0, ws_used = 0;
   for (int gi = 0; gi < n; gi++) {                         // output tiles of the whole launch before any split (same tile rule as below)
     const b2a_convf_t& q = pr[gi];
     if (q.N <= 0 || q.N % 32) continue;                    // rejected by the argument checks below
@@ -848,7 +832,7 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
     // blocks -- a k=3 conv over 390 rows grouped with its 1x1 shortcut -- are 48 tiles with 54 tap steps each)
     const int kchunks = q.cin_pad / TK;
     P.ksplit = 1;
-    if (ksplit_on && sum_base * 2 <= nsm && kchunks >= 4 && ws) {
+    if (sum_base * 2 <= nsm && kchunks >= 4 && ws) {
       int ks = (int)(nsm / sum_base);
       if (ks > 8) ks = 8;
       if (ks > kchunks / 2) ks = kchunks / 2;
@@ -873,20 +857,11 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
     }
     P.tile_begin = tiles_total;
     tiles_total += (int)(base_tiles * P.ksplit);
-    if (gi == 0) first_base = base_tiles;
-    if (base_tiles != first_base || P.ksplit != 1 || q.Cin > CT_MAX / MAXG) can_interleave = false;
     maxR = P.R > maxR ? P.R : maxR; maxBN = P.BN > maxBN ? P.BN : maxBN;
     const int wsz = P.BN * 128 * P.wplanes;
     maxWst = wsz > maxWst ? wsz : maxWst;
   }
   p.ntiles = tiles_total;
-  {
-    static int il = -1;
-    // opt-in: 138 -> 125 us on the warm-L2 microbenchmark of the stage-1 group, but no gain inside the replayed utterance (5.34 vs 5.33 ms)
-    if (il < 0) { const char* e = getenv("B2A_FUSED_INTERLEAVE"); il = (e && e[0] == '1') ? 1 : 0; }
-    p.interleave = (il && n > 1 && can_interleave) ? 1 : 0;
-    p.ct_stride = p.interleave ? CT_MAX / MAXG : CT_MAX;
-  }
   p.a_plane = maxR * 128;
   p.w_stage = maxWst;
   p.acc_ld = acc_tile_ld(maxBN);

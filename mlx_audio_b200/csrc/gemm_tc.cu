@@ -7,7 +7,7 @@
 // padding -- and the weight tile, both into 128B-swizzled shared memory that wgmma consumes through shared-memory descriptors.
 // Two consumer warpgroups each own 64 rows of the 128-row tile and keep their fp32 accumulator in registers; after the K loop the
 // tile goes through shared memory to an epilogue in which each warp streams 32-row x 32-column chunks as whole row segments and
-// fuses bias / activation / LayerScale / residual / scale / accumulate (and, optionally, InstanceNorm partials of the output).
+// fuses bias / activation / LayerScale / residual / scale / accumulate.
 //
 // Precision: activations are stored as TWO bf16 planes (hi = bf16(a), lo = bf16(a - hi)) written by the
 // prologue kernel together with the AdaIN/Snake/LeakyReLU input transform; weights are bf16-exact
@@ -40,7 +40,6 @@ struct TcParams {
   float out_scale; int accumulate;
   float* y; int64_t y_bs, y_ld;
   long long* dbg;                 // optional: clock64 stamps from CTA (0,0,0) (b2a_conv1d_tc_debug)
-  double* stats; int stats_slots; // optional InstanceNorm partials of the OUTPUT: [B][stats_slots][C][2] = (sum, sum of squares) per 32-row group
   // optional: the consumer's A operand, split16 of each final value y.  Either bf16 planes [B][Lout][e_ld] of the next GEMM, or (attn.qh
   // != null) the fp16 attention operands of a fused qkv projection: column n = part * a_hs + head * 64 + d, part 0 = Q (times a_qmul),
   // 1 = K, 2 = V (transposed, keys zero-padded to attn.tkp).
@@ -164,19 +163,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
 
   // ===== epilogue: warp w streams (32-row quarter, 32-column chunk) pairs w, w + 8, ... =====
   const int mul = p.up_s ? p.up_s : 1;
-  const int mt = blockIdx.x;
   for (int pair = warp; pair < 4 * NB; pair += 8) {
     const int quarter = pair & 3, c0 = (pair >> 2) * 32;
     const float* stage = tile + (size_t)(quarter * 32) * LD + c0;
     const int mrow0 = l0 + quarter * 32;
-    if (mrow0 >= p.Mrows) {                                // rows past the end: their statistics slot is an explicit zero
-      if (p.stats) {
-        const int n_ = n0 + c0 + lane, ph_ = p.up_s ? n_ / p.C : 0;
-        double* w = p.stats + ((((int64_t)b * p.stats_slots + (int64_t)(mt * 4 + quarter) * mul + ph_) * p.C) + (n_ - ph_ * p.C)) * 2;
-        w[0] = 0.0; w[1] = 0.0;
-      }
-      continue;
-    }
+    if (mrow0 >= p.Mrows) continue;
     const int n = n0 + c0 + lane;                          // GEMM column of this lane for every row below
     const int ph = p.up_s ? n / p.C : 0;                   // up-sampling phase (uniform over the 32-column chunk)
     const int co = n - ph * p.C;                           // output channel
@@ -200,7 +191,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
     const int64_t rstride = (int64_t)mul * p.res_ld;
     const float osc = p.out_scale;
     const EmitCol ec = emit_col(p, b, n);                  // up-sampling mode never emits (host check), so row = row0 + i below
-    float st1 = 0.f, st2 = 0.f;                            // InstanceNorm partials of the values written below (this lane's column)
     if (i_lo == 0 && i_hi == 32) {
       float rr[32];
       if (rp) {
@@ -230,14 +220,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
 #pragma unroll
         for (int i = 0; i < 32; i++) {
           const float v = epilogue_value(stage[i * LD + lane], bias, p.post_act, p.post_p0, cso, rr[i]);
-          yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
+          yp[i * ystride] = v;
           if (ec.hi) emit_store(ec, row0 + i, v);
         }
       } else {
 #pragma unroll
         for (int i = 0; i < 32; i++) {
           const float v = epilogue_value(stage[i * LD + lane], bias, 0, 0.f, cso, rr[i]);
-          yp[i * ystride] = v; st1 += v; st2 = fmaf(v, v, st2);
+          yp[i * ystride] = v;
           if (ec.hi) emit_store(ec, row0 + i, v);
         }
       }
@@ -249,16 +239,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant
         float rv = rcol ? __ldg(rcol + (int64_t)(half_res ? (row >> 1) : row) * p.res_ld) : 0.f;
         float o = p.accumulate ? ycol[(int64_t)row * p.y_ld] : 0.f;
         const float v = (t * cs + rv) * osc + o;
-        ycol[(int64_t)row * p.y_ld] = v; st1 += v; st2 = fmaf(v, v, st2);
+        ycol[(int64_t)row * p.y_ld] = v;
         if (ec.hi) emit_store(ec, row, v);
       }
       // transposed V: the zero keys that pad Lout to attn.tkp (< 8 rows past the last valid one, so inside this ragged chunk)
       if (ec.hi && ec.step == 1)
         for (int64_t row = p.Lout; row < p.attn.tkp; row++) { ec.hi[row] = 0; ec.lo[row] = 0; }
-    }
-    if (p.stats) {
-      double* w = p.stats + ((((int64_t)b * p.stats_slots + (int64_t)(mt * 4 + quarter) * mul + ph) * p.C) + co) * 2;
-      w[0] = (double)st1; w[1] = (double)st2;
     }
   }
   if (dbg && warp == 0 && lane == 0) p.dbg[5] = clock64();
@@ -377,7 +363,7 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
                                  int32_t taps, const int32_t* shifts_host, int32_t Cout, int32_t Lout, const float* bias,
                                  int32_t post_act, float post_p0, const float* cscale, int64_t cscale_bs, const float* res,
                                  int64_t res_bs, int64_t res_ld, int32_t res_div, float out_scale, int32_t accumulate, float* y,
-                                 int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop, double* stats_ws, int32_t stats_slots,
+                                 int64_t y_bs, int64_t y_ld, int32_t up_stride, int32_t up_crop,
                                  void* emit_hi, void* emit_lo, int64_t emit_ld, void* attn_ws, int32_t attn_heads, float attn_scale,
                                  void* stream) {
   B2A_CHECK_ARG(a_hi && w_bf16 && y && shifts_host, "null pointer");
@@ -421,21 +407,12 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
   p.res = res; p.res_bs = res_bs; p.res_ld = res_ld; p.res_div = res_div; p.out_scale = out_scale; p.accumulate = accumulate;
   p.y = y; p.y_bs = y_bs; p.y_ld = y_ld;
   p.dbg = g_dbg;
-  p.stats = stats_ws; p.stats_slots = stats_slots;
   const int stage_bytes = TM * 128 * p.planes + p.BN * 128 * p.wplanes;
   const size_t tile_bytes = (size_t)TM * (p.BN + 8) * 4;
   // One CTA per SM (the epilogue's register arrays put a CTA at ~125 registers per thread): as many operand stages as fit.
   p.stages = (200 * 1024) / stage_bytes; if (p.stages > 6) p.stages = 6; if (p.stages < 2) p.stages = 2;
   const size_t ring = (size_t)p.stages * stage_bytes;
   const size_t smem = (ring > tile_bytes ? ring : tile_bytes) + 1024 /*align slack*/ + 2 * p.stages * 8 + 64;
-
-  if (stats_ws) {
-    const int need = cdiv(p.Mrows, TM) * 4 * (up_stride ? up_stride : 1);
-    if (stats_slots != need) {
-      b2a_set_error("b2a_conv1d_tc: fused output statistics need %d slots (got %d)", need, stats_slots);
-      return B2A_E_UNSUPPORTED;
-    }
-  }
 
   CUtensorMap mh, ml, mw, mwl;
   uint64_t adims[3] = {(uint64_t)cin_pad, (uint64_t)L, (uint64_t)B};

@@ -441,169 +441,6 @@ __global__ void __launch_bounds__(AD_THREADS) attn_decode_kernel(const AdParams 
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Single-token decode: q/k RMSNorm + rotary + cache append + GQA attention in ONE launch.  One CTA per (kv head, batch): warp 0
-// normalises / rotates k and appends it, warp 1 appends v, warps 2.. prepare the G = Hq/Hkv query heads that share this kv
-// head; then all 8 warps stride the cache rows once and score them against all G queries (each K / V row is read once for
-// the whole group), softmax per query, P V, cross-warp reduce.
-struct FdParams {
-  const float* qkv; int64_t qkv_bs;                // [B, (Hq+2Hkv) D], one token per batch row
-  int B, Hq, Hkv;
-  const float* qn; const float* kn; float eps;
-  const int* pos3; const int* base_dev; int base_host; int sec_h, sec_w; float theta;
-  float* kc; float* vc; int64_t c_bs, c_ss; int smax;
-  float* o; int64_t o_bs; float scale; const int* kv_start;
-  const int* base_rows; const int* slot;           // [B] per-row base (negative: no write, zero output) and cache batch index
-};
-
-template <int D, int G>
-__global__ void __launch_bounds__(256) attn_decode_fused_kernel(const FdParams p) {
-  constexpr int E = D / 32, NW = 8;
-  extern __shared__ __align__(16) float fsm[];       // [G][max_k] scores | reused as [NW][G][D] partials
-  __shared__ __align__(16) float qs[G][D];
-  __shared__ float redm[G][NW], reds[G][NW];
-  const int hk = blockIdx.x, b = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  pdl_launch_dependents();
-  pdl_wait();
-  const int base = p.base_rows ? p.base_rows[b] : (p.base_dev ? *p.base_dev : p.base_host);
-  const int klen = min(base + 1, p.smax);
-  const int k0 = p.kv_start ? p.kv_start[b] : 0;
-  const int cb = p.slot ? p.slot[b] : b;
-  const float* row = p.qkv + (int64_t)b * p.qkv_bs;
-  float* kb = p.kc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
-  float* vb = p.vc + (int64_t)cb * p.c_bs + (int64_t)hk * D;
-  // ---- phase A: prepare q (G heads), k, v
-  if (warp < G + 2) {
-    const bool is_v = warp == 1, is_k = warp == 0;
-    const int head = is_k ? p.Hq + hk : (is_v ? p.Hq + p.Hkv + hk : hk * G + (warp - 2));
-    const float* src = row + (int64_t)head * D;
-    float v[E];
-#pragma unroll
-    for (int j = 0; j < E; j++) v[j] = src[lane + 32 * j];
-    if (is_v) {
-      if (base >= 0 && base < p.smax) {
-#pragma unroll
-        for (int j = 0; j < E; j++) vb[(int64_t)base * p.c_ss + lane + 32 * j] = v[j];
-      }
-    } else {
-      const float* nw = is_k ? p.kn : p.qn;
-      if (nw) {
-        float ss = 0.f;
-#pragma unroll
-        for (int j = 0; j < E; j++) ss = fmaf(v[j], v[j], ss);
-        ss = warp_sum(ss);
-        const float rinv = rsqrtf(ss / (float)D + p.eps);
-#pragma unroll
-        for (int j = 0; j < E; j++) v[j] = v[j] * rinv * __ldg(nw + lane + 32 * j);
-      }
-      float o[E];
-#pragma unroll
-      for (int j = 0; j < E / 2; j++) {
-        const int i = lane + 32 * j;
-        int axis = 0;
-        if (i % 3 == 1 && i < 3 * p.sec_h) axis = 1; else if (i % 3 == 2 && i < 3 * p.sec_w) axis = 2;
-        const int pos = p.pos3 ? p.pos3[(int64_t)axis * p.B + b] : base;
-        const double inv = exp2(-(double)(2 * i) / (double)D * log2((double)p.theta));
-        double sn, cs;
-        sincos((double)pos * inv, &sn, &cs);
-        const float c = (float)cs, sf = (float)sn;
-        o[j] = v[j] * c - v[j + E / 2] * sf;
-        o[j + E / 2] = v[j + E / 2] * c + v[j] * sf;
-      }
-      if (is_k) {
-        if (base >= 0 && base < p.smax) {
-#pragma unroll
-          for (int j = 0; j < E; j++) kb[(int64_t)base * p.c_ss + lane + 32 * j] = o[j];
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < E; j++) qs[warp - 2][lane + 32 * j] = o[j] * p.scale;
-      }
-    }
-  }
-  __syncthreads();                                    // the appended K / V row is visible to the whole CTA from here on
-  // ---- phase B: scores
-  float qv[G][E];
-#pragma unroll
-  for (int g = 0; g < G; g++)
-#pragma unroll
-    for (int j = 0; j < E; j++) qv[g][j] = qs[g][lane * E + j];
-  float mloc[G];
-#pragma unroll
-  for (int g = 0; g < G; g++) mloc[g] = -INFINITY;
-  const int max_k = p.smax;
-  for (int j = k0 + warp; j < klen; j += NW) {
-    const float* kr = kb + (int64_t)j * p.c_ss + lane * E;
-    float kv[E];
-    if constexpr (E == 4) { float4 t = *reinterpret_cast<const float4*>(kr); kv[0] = t.x; kv[1] = t.y; kv[2] = t.z; kv[3] = t.w; }
-    else { float2 t = *reinterpret_cast<const float2*>(kr); kv[0] = t.x; kv[1] = t.y; }
-#pragma unroll
-    for (int g = 0; g < G; g++) {
-      float d = 0.f;
-#pragma unroll
-      for (int e = 0; e < E; e++) d = fmaf(qv[g][e], kv[e], d);
-      d = warp_sum(d);
-      if (lane == 0) fsm[g * max_k + j] = d;
-      mloc[g] = fmaxf(mloc[g], d);
-    }
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int g = 0; g < G; g++) redm[g][warp] = mloc[g];
-  }
-  __syncthreads();
-  float tot[G];
-#pragma unroll
-  for (int g = 0; g < G; g++) {
-    float gm = redm[g][0];
-#pragma unroll
-    for (int w = 1; w < NW; w++) gm = fmaxf(gm, redm[g][w]);
-    float sl = 0.f;
-    for (int j = k0 + (int)threadIdx.x; j < klen; j += 256) { float e = __expf(fsm[g * max_k + j] - gm); fsm[g * max_k + j] = e; sl += e; }
-    sl = warp_sum(sl);
-    if (lane == 0) reds[g][warp] = sl;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int g = 0; g < G; g++) { float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < NW; w++) t += reds[g][w];
-    tot[g] = t; }
-  // ---- phase C: P V
-  float acc[G][E];
-#pragma unroll
-  for (int g = 0; g < G; g++)
-#pragma unroll
-    for (int e = 0; e < E; e++) acc[g][e] = 0.f;
-  for (int j = k0 + warp; j < klen; j += NW) {
-    const float* vr = vb + (int64_t)j * p.c_ss + lane * E;
-    float vv[E];
-    if constexpr (E == 4) { float4 t = *reinterpret_cast<const float4*>(vr); vv[0] = t.x; vv[1] = t.y; vv[2] = t.z; vv[3] = t.w; }
-    else { float2 t = *reinterpret_cast<const float2*>(vr); vv[0] = t.x; vv[1] = t.y; }
-#pragma unroll
-    for (int g = 0; g < G; g++) {
-      const float pj = fsm[g * max_k + j];
-#pragma unroll
-      for (int e = 0; e < E; e++) acc[g][e] = fmaf(pj, vv[e], acc[g][e]);
-    }
-  }
-  __syncthreads();
-  float* part = fsm;                                  // [NW][G][D]
-#pragma unroll
-  for (int g = 0; g < G; g++)
-#pragma unroll
-    for (int e = 0; e < E; e++) part[(warp * G + g) * D + lane * E + e] = acc[g][e];
-  __syncthreads();
-  for (int i = threadIdx.x; i < G * D; i += 256) {
-    const int g = i / D, d = i % D;
-    float v = 0.f;
-#pragma unroll
-    for (int w = 0; w < NW; w++) v += part[(w * G + g) * D + d];
-    p.o[(int64_t)b * p.o_bs + (int64_t)(hk * G + g) * D + d] = tot[g] > 0.f ? v / tot[g] : 0.f;
-  }
-}
-
 __global__ void swiglu_kernel(const float* x, int64_t x_ld, int64_t rows, int I, int interleaved, float* y, int64_t y_ld) {
   const int64_t total = rows * I;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -688,9 +525,7 @@ extern "C" int32_t b2a_gemv_bf16(const float* x, int64_t x_ld, int32_t M, int32_
                (const char*)prefetch, prefetch ? prefetch_bytes : 0};
   const int grid = (N + GV_ROWS - 1) / GV_ROWS;
   cudaStream_t st = (cudaStream_t)stream;
-  static int wide_on = -1;
-  if (wide_on < 0) { const char* e = getenv("B2A_GEMV_WIDE"); wide_on = (e && e[0] == '0') ? 0 : 1; }
-  const bool wide = wide_on && M > 2 && (K >> 3) % (GV_THREADS / 32) == 0;
+  const bool wide = M > 2 && (K >> 3) % (GV_THREADS / 32) == 0;
   const int gridw = (N + GW_ROWS - 1) / GW_ROWS;
   if (M == 1) b2a_launch_pdl(gemv_bf16_kernel<1>, dim3(grid), dim3(GV_THREADS), 0, st, p);
   else if (M == 2) b2a_launch_pdl(gemv_bf16_kernel<2>, dim3(grid), dim3(GV_THREADS), 0, st, p);
@@ -744,33 +579,6 @@ extern "C" int32_t b2a_attn_decode(const float* q, int64_t q_bs, int64_t q_ss, c
   } else {
     if (sm > 48 * 1024) cudaFuncSetAttribute(attn_decode_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     b2a_launch_pdl(attn_decode_kernel<32>, grid, dim3(AD_THREADS), sm, st, p);
-  }
-  B2A_CHECK_LAUNCH();
-  return B2A_OK;
-}
-
-extern "C" int32_t b2a_attn_decode_fused(const float* qkv, int64_t qkv_bs, int32_t B, int32_t Hq, int32_t Hkv, int32_t D,
-                                         const float* q_norm_w, const float* k_norm_w, float eps, const int32_t* pos3,
-                                         const int32_t* base_dev, int32_t base_host, int32_t sec_h, int32_t sec_w, float theta,
-                                         float* k_cache, float* v_cache, int64_t c_bs, int64_t c_ss, int32_t smax, float scale,
-                                         const int32_t* kv_start, float* out, int64_t o_bs, const int32_t* base_rows,
-                                         const int32_t* slot, void* stream) {
-  B2A_CHECK_ARG((D == 64 || D == 128) && Hq == 2 * Hkv, "fused decode attention: head_dim 64/128 and a 2:1 GQA group");
-  B2A_CHECK_ARG(B > 0 && smax > 0 && smax <= 24 * 1024, "bad shape (cache rows <= 24576)");
-  B2A_CHECK_ARG(c_ss % 4 == 0 && c_bs % 4 == 0 && ((uintptr_t)k_cache & 15) == 0 && ((uintptr_t)v_cache & 15) == 0, "cache rows must be 16-byte aligned");
-  FdParams p{qkv, qkv_bs, B, Hq, Hkv, q_norm_w, k_norm_w, eps, pos3, base_dev, base_host, sec_h, sec_w, theta, k_cache, v_cache, c_bs, c_ss,
-             smax, out, o_bs, scale, kv_start, base_rows, slot};
-  size_t floats = (size_t)2 * smax;
-  if (floats < (size_t)8 * 2 * D) floats = (size_t)8 * 2 * D;
-  const size_t sm = floats * sizeof(float);
-  dim3 grid(Hkv, B);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (D == 128) {
-    if (sm > 48 * 1024) cudaFuncSetAttribute(attn_decode_fused_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    b2a_launch_pdl(attn_decode_fused_kernel<128, 2>, grid, dim3(256), sm, st, p);
-  } else {
-    if (sm > 48 * 1024) cudaFuncSetAttribute(attn_decode_fused_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    b2a_launch_pdl(attn_decode_fused_kernel<64, 2>, grid, dim3(256), sm, st, p);
   }
   B2A_CHECK_LAUNCH();
   return B2A_OK;

@@ -158,14 +158,6 @@ extern "C" int32_t b2a_adain_coeffs(const float* x, int64_t x_bs, int64_t x_ld, 
   return B2A_OK;
 }
 
-extern "C" int32_t b2a_adain_coeffs_from_partials(const double* partials, int32_t nslots, int32_t B, int32_t L, int32_t C, const float* gb,
-                                                  float eps, float* scale, float* shift, void* stream) {
-  B2A_CHECK_ARG(partials && scale && shift && B > 0 && L > 0 && C > 0 && nslots > 0, "bad pointers/shape");
-  adain_final_kernel<<<cdiv((int64_t)B * C, 8), 256, 0, (cudaStream_t)stream>>>(partials, nslots, L, C, gb, eps, scale, shift, B);
-  B2A_CHECK_LAUNCH();
-  return B2A_OK;
-}
-
 extern "C" int32_t b2a_channel_stats(const float* x, int64_t x_bs, int64_t x_ld, int32_t B, int32_t L, int32_t C, int64_t* const* dst,
                                      const int64_t* dst_bs, int32_t n_dst, void* stream) {
   B2A_CHECK_ARG(x && dst && dst_bs && B > 0 && L > 0 && C > 0 && n_dst >= 1 && n_dst <= 4, "bad pointers/shape (1..4 destinations)");

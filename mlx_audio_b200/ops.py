@@ -210,10 +210,8 @@ def pack_linear(w: torch.Tensor, bias=None, device="cuda") -> ConvW:
 
 def conv1d(x: torch.Tensor, cw: ConvW, *, stride=1, dilation=1, pad_left=0, lout=None, pad_mode=0,
            pre: Optional[Pre] = None, post_act=0, post_p0=0.0, cscale=None, res=None, res_div=1,
-           out_scale=1.0, out=None, accumulate=False, transpose=False, stats=False, emit: Optional[Pre] = None):
-    """b2a_conv1d_cl / b2a_convtr1d_cl.  For ``transpose`` ``pad_left`` is the left crop of the scatter output.
-    ``stats=True`` returns (y, partials): InstanceNorm partial sums of y from the tensor-core epilogue for ``adain_coeffs(partials=)``,
-    or (y, None) when the layer does not run on that path."""
+           out_scale=1.0, out=None, accumulate=False, transpose=False, emit: Optional[Pre] = None):
+    """b2a_conv1d_cl / b2a_convtr1d_cl.  For ``transpose`` ``pad_left`` is the left crop of the scatter output."""
     if isinstance(x, Planes):                      # operand already split by its producer (conv1d(..., emit=...)): tensor-core path only
         B, L, cin = x.shape
         if (cin != cw.cin or pre is not None or not _tc_eligible(cw, L, stride, transpose, pad_mode, dilation) or x.hi.shape[2] != cw.cin_pad
@@ -222,7 +220,7 @@ def conv1d(x: torch.Tensor, cw: ConvW, *, stride=1, dilation=1, pad_left=0, lout
         if lout is None:
             lout = (L + 2 * pad_left - dilation * (cw.K - 1) - 1) // stride + 1
         return _conv1d_tc(x, cw, dilation, pad_left, lout, None, post_act, post_p0, cscale, res, res_div, out_scale, out, accumulate,
-                          up_stride=stride if transpose else 0, stats=stats)
+                          up_stride=stride if transpose else 0)
     _chk3(x, "conv1d x")
     B, L, cin = x.shape
     if cin != cw.cin:
@@ -234,15 +232,15 @@ def conv1d(x: torch.Tensor, cw: ConvW, *, stride=1, dilation=1, pad_left=0, lout
             lout = (L + 2 * pad_left - dilation * (cw.K - 1) - 1) // stride + 1
     # Tiny GEMMs (a few rows: ALBERT at T = 130, decode-time prefills) are latency chains, not throughput problems: the fused kernel's
     # converter -> MMA -> split-K fix-up chain measured 30-40 us per launch there against ~14 us for the pre-split planes + TMA pipeline.
-    small_gemm = SMALL_GEMM_SPLIT_PATH[0] and cw.K == 1 and B * L <= 256 and _tc_eligible(cw, L, stride, transpose, pad_mode, dilation)
+    small_gemm = cw.K == 1 and B * L <= 256 and _tc_eligible(cw, L, stride, transpose, pad_mode, dilation)
     if FUSED_DISPATCH[0] and emit is None and not small_gemm and fused_eligible(x, cw, stride, dilation, transpose, pad_mode, out, res):
         y = conv_fused(FusedProblem(x, cw, stride=stride, dilation=dilation, pad_left=pad_left, lout=lout, pre=pre, post_act=post_act,
                                     post_p0=post_p0, cscale=cscale, res=res, res_div=res_div, out_scale=out_scale, out=out,
                                     accumulate=accumulate, transpose=transpose))[0]
-        return (y, None) if stats else y
+        return y
     if _tc_eligible(cw, L, stride, transpose, pad_mode, dilation):
         return _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, res, res_div, out_scale, out, accumulate,
-                          up_stride=stride if transpose else 0, stats=stats)
+                          up_stride=stride if transpose else 0)
     planes = None
     if emit is not None:
         if not emit_eligible(cw, x, lout, stride, dilation, transpose) or res is not None or cscale is not None or accumulate or post_act or out is not None:
@@ -284,7 +282,7 @@ def conv1d(x: torch.Tensor, cw: ConvW, *, stride=1, dilation=1, pad_left=0, lout
     _call("conv" if cw.groups == 1 and cw.cin * cw.K >= 64 else "other", fn, 1, C.byref(p), _stream())
     if planes is not None:
         return planes
-    return (out, None) if stats else out
+    return out
 
 
 def emit_eligible(cw: "ConvW", x: torch.Tensor, lout: int, stride: int = 1, dilation: int = 1, transpose: bool = False) -> bool:
@@ -313,11 +311,6 @@ def prep_bf16(x: torch.Tensor, pre: Optional[Pre], cpad: int, planes: int = 2, f
     return hi, lo
 
 
-# InstanceNorm partials from the conv epilogue: correct (tests/test_tc_gpu.py) but opt-in: the per-32-row float64 slots make the
-# coefficient kernel strided and lengthen the epilogue that sits on the critical path.
-TC_STATS = [os.environ.get("B2A_TC_STATS", "0") != "0"]
-
-
 def _new_planes(B: int, L: int, C: int, device) -> Planes:
     """Uninitialised bf16 planes [B, L, C] for a producer to fill (lo only in "x2" mode)."""
     return Planes(torch.empty(B, L, C, device=device, dtype=torch.bfloat16),
@@ -335,7 +328,7 @@ class AttnPlanes:
 
 
 def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, res, res_div, out_scale, out, accumulate,
-               up_stride=0, stats=False, emit: Optional[Planes] = None, attn: Optional[AttnPlanes] = None, attn_scale=0.0):
+               up_stride=0, emit: Optional[Planes] = None, attn: Optional[AttnPlanes] = None, attn_scale=0.0):
     if isinstance(x, Planes):
         B, L, _ = x.shape
         hi, lo = x.hi, x.lo
@@ -360,17 +353,12 @@ def _conv1d_tc(x, cw, dilation, pad_left, lout, pre, post_act, post_p0, cscale, 
     if res is not None:
         _chk3(res, "conv1d res")
         r, r_bs, r_ld = res.data_ptr(), (res.stride(0) if res.shape[0] == B else 0), res.stride(1)
-    ws, slots = None, 0
-    if stats and TC_STATS[0]:          # InstanceNorm partials of the output straight from the epilogue (persistent kernel only)
-        mrows = max(L + taps - 1, -(-(lout + pad_left) // up_stride)) if up_stride else lout      # b2a_conv1d_tc's GEMM rows
-        slots = -(-mrows // 128) * 4 * max(1, up_stride)
-        ws = torch.empty(B, slots, cw.cout, 2, device=hi.device, dtype=torch.float64)
     _call("conv_tc", _lib.lib().b2a_conv1d_tc, 1, hi.data_ptr(), _p(lo), int(cw.f16), B, L, cw.cin_pad, w_tc.data_ptr(), _p(w_lo), taps, shifts, n_total, lout,
           _p(cw.bias), post_act, post_p0, cs, cs_bs, r, r_bs, r_ld, res_div, out_scale, int(accumulate), out.data_ptr(), out.stride(0),
-          out.stride(1), up_stride, pad_left if up_stride else 0, _p(ws), slots,
+          out.stride(1), up_stride, pad_left if up_stride else 0,
           None if emit is None else emit.hi.data_ptr(), None if emit is None else _p(emit.lo), 0 if emit is None else emit.hi.stride(1),
           None if attn is None else attn.ws.data_ptr(), 0 if attn is None else attn.H, float(attn_scale), _stream())
-    return (out, ws) if stats else out
+    return out
 
 
 CL_PATHS = {1: "linear_rows", 2: "narrow", 3: "dense", 4: "dw_tiled4", 5: "dw_tiled", 6: "dw", 7: "convtr_dense", 8: "convtr_dw"}
@@ -421,7 +409,6 @@ def fused_dispatch(on: bool = True):
         yield
     finally:
         FUSED_DISPATCH[0] = old
-SMALL_GEMM_SPLIT_PATH = [os.environ.get("B2A_SMALL_GEMM_SPLIT", "1") != "0"]
 FUSED_WS_BYTES = 16 << 20
 _FUSED_WS = {}
 
@@ -781,18 +768,12 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
     return ws
 
 
-def adain_coeffs(x: torch.Tensor, gb: Optional[torch.Tensor], eps=1e-5, partials: Optional[torch.Tensor] = None):
-    """InstanceNorm stats of x [B,L,C] folded with AdaIN (gamma|beta) [B,2C] -> (scale, shift) [B,C].  ``partials`` [B,slots,C,2]
-    float64 from ``conv1d(..., stats=True)`` skips the statistics pass over x."""
+def adain_coeffs(x: torch.Tensor, gb: Optional[torch.Tensor], eps=1e-5):
+    """InstanceNorm stats of x [B,L,C] folded with AdaIN (gamma|beta) [B,2C] -> (scale, shift) [B,C]."""
     _chk3(x, "adain_coeffs x")
     B, L, Cc = x.shape
     scale = torch.empty(B, Cc, device=x.device, dtype=torch.float32)
     shift = torch.empty(B, Cc, device=x.device, dtype=torch.float32)
-    if partials is not None:
-        assert partials.dtype == torch.float64 and partials.is_contiguous() and partials.shape[0] == B and partials.shape[2] == Cc
-        _call("adain_stats", _lib.lib().b2a_adain_coeffs_from_partials, 1, partials.data_ptr(), partials.shape[1], B, L, Cc, _p(gb), eps,
-              scale.data_ptr(), shift.data_ptr(), _stream())
-        return scale, shift
     ws = _workspace(_lib.lib().b2a_adain_ws_bytes(B, L, Cc), x.device)
     _call("adain_stats", _lib.lib().b2a_adain_coeffs, 2, x.data_ptr(), x.stride(0), x.stride(1), B, L, Cc, _p(gb), eps,
                                            scale.data_ptr(), shift.data_ptr(), ws.data_ptr(), _stream())
@@ -1135,23 +1116,6 @@ def attn_prefill(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, 
     _call("attention", _lib.lib().b2a_attn_prefill, 1, q.data_ptr(), q.stride(0), q.stride(1), k_cache.data_ptr(), v_cache.data_ptr(),
           k_cache.stride(0), k_cache.stride(1), out.data_ptr(), out.stride(0), out.stride(1), B, S, n_heads, n_kv, head_dim, scale,
           _p(base_dev), base, _p(kv_start), max_k, _p(_rows_i32(base_rows, B)), _p(_rows_i32(slot, B)), _stream())
-    return out
-
-
-def attn_decode_fused(qkv: torch.Tensor, n_heads: int, n_kv: int, head_dim: int, k_cache: torch.Tensor, v_cache: torch.Tensor, *, scale: float,
-                      q_norm=None, k_norm=None, eps: float = 1e-6, pos3=None, base_dev=None, base: int = 0, mrope=(0, 0),
-                      theta: float = 10000.0, kv_start=None, out=None, base_rows=None, slot=None) -> torch.Tensor:
-    """Single-token decode step: qkv [B,(Hq+2Hkv)D] -> attention output [B,Hq*D]; k/v appended to the caches at row ``base``
-    (``base_rows`` / ``slot`` as in ``qknorm_rope_cache``)."""
-    assert qkv.dim() == 2 and qkv.stride(1) == 1 and n_heads == 2 * n_kv and k_cache.stride() == v_cache.stride()
-    B = qkv.shape[0]
-    if out is None:
-        out = torch.empty(B, n_heads * head_dim, device=qkv.device, dtype=torch.float32)
-    assert pos3 is None or (pos3.dtype == torch.int32 and pos3.is_contiguous() and pos3.numel() == 3 * B)
-    _call("attention", _lib.lib().b2a_attn_decode_fused, 1, qkv.data_ptr(), qkv.stride(0), B, n_heads, n_kv, head_dim, _p(q_norm), _p(k_norm),
-          eps, _p(pos3), _p(base_dev), base, mrope[0], mrope[1], theta, k_cache.data_ptr(), v_cache.data_ptr(), k_cache.stride(0),
-          k_cache.stride(1), k_cache.shape[1], scale, _p(kv_start), out.data_ptr(), out.stride(0), _p(_rows_i32(base_rows, B)),
-          _p(_rows_i32(slot, B)), _stream())
     return out
 
 

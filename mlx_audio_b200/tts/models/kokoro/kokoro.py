@@ -298,10 +298,10 @@ class Model:
         L = x.shape[1]
         if blk["up"]:
             r = ops.conv1d(x, blk["pool"], stride=2, pad_left=1, lout=2 * L, pre=pre1, transpose=True)
-            r, part = ops.conv1d(r, blk["conv1"], pad_left=1, stats=True)
+            r = ops.conv1d(r, blk["conv1"], pad_left=1)
         else:
-            r, part = ops.conv1d(x, blk["conv1"], pad_left=1, pre=pre1, stats=True)
-        s2, h2 = ops.adain_coeffs(r, self._gb(blk["name"] + ".norm2").contiguous(), partials=part)
+            r = ops.conv1d(x, blk["conv1"], pad_left=1, pre=pre1)
+        s2, h2 = ops.adain_coeffs(r, self._gb(blk["name"] + ".norm2").contiguous())
         sc = ops.conv1d(x, blk["sc"]) if "sc" in blk else x
         return ops.conv1d(r, blk["conv2"], pad_left=1, pre=Pre(s2, h2, ACT["lrelu"], 0.2), res=sc,
                           res_div=2 if blk["up"] else 1, out_scale=1.0 / math.sqrt(2.0), out=out)
@@ -310,12 +310,11 @@ class Model:
         """AdaINResBlock1 (istftnet.py:341-396) on x [1,L,C].  ``defer_last`` returns a closure issuing the final conv
         (the one that writes / accumulates into ``out``) so parallel branches can serialise only that step."""
         k = blk["k"]
-        xpart = None                                      # InstanceNorm partials of x when its producer (the previous c2) emitted them
         for j, d in enumerate(blk["dils"]):
-            s1, h1 = ops.adain_coeffs(x, self._gb(f"{blk['name']}.adain1.{j}").contiguous(), partials=xpart)
+            s1, h1 = ops.adain_coeffs(x, self._gb(f"{blk['name']}.adain1.{j}").contiguous())
             a, ia = blk["a1"][j]
-            xt, tpart = ops.conv1d(x, blk["c1"][j], dilation=d, pad_left=(k * d - d) // 2, pre=Pre(s1, h1, ACT["snake"], 0.0, a, ia), stats=True)
-            s2, h2 = ops.adain_coeffs(xt, self._gb(f"{blk['name']}.adain2.{j}").contiguous(), partials=tpart)
+            xt = ops.conv1d(x, blk["c1"][j], dilation=d, pad_left=(k * d - d) // 2, pre=Pre(s1, h1, ACT["snake"], 0.0, a, ia))
+            s2, h2 = ops.adain_coeffs(xt, self._gb(f"{blk['name']}.adain2.{j}").contiguous())
             a, ia = blk["a2"][j]
             last = j == len(blk["dils"]) - 1
             if last and defer_last:
@@ -327,7 +326,7 @@ class Model:
                 x = ops.conv1d(xt, blk["c2"][j], pad_left=(k - 1) // 2, pre=Pre(s2, h2, ACT["snake"], 0.0, a, ia), res=x,
                                out=out, out_scale=out_scale, accumulate=accumulate)
             else:
-                x, xpart = ops.conv1d(xt, blk["c2"][j], pad_left=(k - 1) // 2, pre=Pre(s2, h2, ACT["snake"], 0.0, a, ia), res=x, stats=True)
+                x = ops.conv1d(xt, blk["c2"][j], pad_left=(k - 1) // 2, pre=Pre(s2, h2, ACT["snake"], 0.0, a, ia), res=x)
         return x
 
 

@@ -11,7 +11,6 @@ CUDA graph (see qwen3_tts.py).  Prefill (S >= 17 rows) runs the same layers on t
 """
 from __future__ import annotations
 
-import os
 from typing import Optional
 
 import torch
@@ -21,9 +20,6 @@ from .config import Qwen3TTSTalkerCodePredictorConfig, Qwen3TTSTalkerConfig
 
 GEMV_MAX_ROWS = 16
 PREFILL_TC_MIN_ROWS = 64          # prefills of at least this many rows run attention on b2a_attn_prefill (one full query tile)
-FUSED_DECODE = [os.environ.get("B2A_LM_FUSED", "0") != "0"]       # S = 1: qk-norm + rope + cache append + attention in one launch
-# (8 CTAs walking the cache lose to 384 warps + 16 CTAs at small batch; kept for B >= 8)
-PREFETCH = [os.environ.get("B2A_LM_PREFETCH", "1") != "0"]      # pull the next projection's weights into L2 from the current GEMV
 
 
 def _interleave(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
@@ -65,8 +61,9 @@ class _DecoderStack:
             self.vc = torch.zeros(shape, device=self.device, dtype=torch.float32)
 
     def _proj(self, x2, cw, norm_w=None, swiglu=False, res=None, nxt=None):
+        # nxt: the next projection, whose weights the GEMV pulls into L2 while it streams its own
         if x2.shape[0] <= GEMV_MAX_ROWS and ops.gemv_eligible(cw):
-            return ops.gemv(x2, cw, norm_w=norm_w, norm_eps=self.eps, swiglu=swiglu, res=res, prefetch=nxt if PREFETCH[0] else None)
+            return ops.gemv(x2, cw, norm_w=norm_w, norm_eps=self.eps, swiglu=swiglu, res=res, prefetch=nxt)
         h = ops.layernorm(x2, norm_w, None, eps=self.eps, rms=True) if norm_w is not None else x2
         y = ops.linear(h, cw, res=None if swiglu else res)
         return ops.swiglu(y, interleaved=True) if swiglu else y
@@ -88,17 +85,12 @@ class _DecoderStack:
         for li, lw in enumerate(self.layers):
             nxt_qkv = self.layers[li + 1]["qkv"] if li + 1 < len(self.layers) else tail
             qkv = self._proj(x2, lw["qkv"], norm_w=lw["n1"], nxt=lw["o"])
-            if S == 1 and hq == 2 * hk and hd in (64, 128) and FUSED_DECODE[0] and pos_shift is None:
-                a = ops.attn_decode_fused(qkv, hq, hk, hd, self.kc[li], self.vc[li], scale=hd ** -0.5, q_norm=lw["qn"], k_norm=lw["kn"],
-                                          eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
-                                          kv_start=kv_start, **rows)
-            else:
-                q = ops.qknorm_rope_cache(qkv.view(B, S, -1), hq, hk, hd, self.kc[li], self.vc[li], q_norm=lw["qn"], k_norm=lw["kn"],
-                                          eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
-                                          pos_shift=pos_shift, **rows)
-                attn = ops.attn_prefill if prefill_tc else ops.attn_decode
-                a = attn(q, self.kc[li], self.vc[li], hq, hk, hd, scale=hd ** -0.5, base_dev=base_dev, base=base, kv_start=kv_start,
-                         max_k=max_k, **rows)
+            q = ops.qknorm_rope_cache(qkv.view(B, S, -1), hq, hk, hd, self.kc[li], self.vc[li], q_norm=lw["qn"], k_norm=lw["kn"],
+                                      eps=self.eps, pos3=pos3, base_dev=base_dev, base=base, mrope=self.mrope, theta=self.theta,
+                                      pos_shift=pos_shift, **rows)
+            attn = ops.attn_prefill if prefill_tc else ops.attn_decode
+            a = attn(q, self.kc[li], self.vc[li], hq, hk, hd, scale=hd ** -0.5, base_dev=base_dev, base=base, kv_start=kv_start,
+                     max_k=max_k, **rows)
             x2 = self._proj(a.view(B * S, hq * hd), lw["o"], res=x2, nxt=lw["gu"])
             m = self._proj(x2, lw["gu"], norm_w=lw["n2"], swiglu=True, nxt=lw["down"])
             x2 = self._proj(m, lw["down"], res=x2, nxt=nxt_qkv)

@@ -18,7 +18,7 @@ from mlx_audio_b200 import build
 
 SRC = os.path.join(build.CSRC, "conv_fused.cu")
 # (spill stores, spill loads) in bytes per instantiation: DBG = false is the production kernel, DBG = true the timeline build
-SPILL_BOUND = {"conv_fused_kernelILb0E": (64, 84), "conv_fused_kernelILb1E": (192, 224)}
+SPILL_BOUND = {"conv_fused_kernelILb0E": (44, 44), "conv_fused_kernelILb1E": (128, 156)}
 VARIANTS = 4 * 2                      # mma_tile instantiations per kernel: NB = 1..4 x (bf16, fp16)
 
 

@@ -161,7 +161,7 @@ def _nsm():
     return _lib.lib().b2a_device_sm_count()
 
 
-def _plan(cases, nsm, ws_bytes, ksplit_on=True) -> Plan:
+def _plan(cases, nsm, ws_bytes) -> Plan:
     """b2a_conv1d_fused's tiling: heaviest problem first (taps x cin_pad), K split when the whole launch has at most nsm / 2 output
     tiles and the problem at least 4 K chunks, each split problem's partial tiles and counters placed in the workspace in that order."""
     n = len(cases)
@@ -179,7 +179,7 @@ def _plan(cases, nsm, ws_bytes, ksplit_on=True) -> Plan:
         c = cases[i]
         kchunks = c.cin_pad // TK
         k = 1
-        if ksplit_on and sum_base * 2 <= nsm and kchunks >= 4 and ws_bytes:
+        if sum_base * 2 <= nsm and kchunks >= 4 and ws_bytes:
             k = min(nsm // sum_base, 8, kchunks // 2)
             k = k if k >= 2 else 1
         kper = -(-kchunks // k)
@@ -615,82 +615,42 @@ def test_split_k_workspace_fallback_and_rearm(small_ws):
 
 
 # --------------------------------------------------------------------------------------------------------------- per-process switches
-# B2A_FUSED_INTERLEAVE / _KSPLIT / _PDL are read once per process, so each runs in a child process that writes its results to a file.
-_IL_GROUP = [Case(f"il_k{k}", 2, 1000, 192, 128, k, dil=3, pre="stats_gb", act="snake", stats_out=True) for k in (3, 7, 11)]
-_KS_CASE = Case("ks_off_split", 1, 200, 512, 128, 3, pre="stats", act="lrelu")
+# B2A_FUSED_PDL is read once per process, so it runs in a child process that writes its results to a file.
 _PDL_CHAIN = Case("pdl_chain", 1, 300, 256, 256, 3)
 
 
-def _scenario(which: str) -> dict:
+def _pdl_chain() -> dict:
+    """A dependent chain of split-K launches (6 output tiles, 4 K chunks)."""
     from mlx_audio_b200 import ops
     ops.TC_MODE[0] = "x2"
     out = {}
-    if which == "interleave":
-        probs = [Prob(ops, c) for c in _IL_GROUP]
-        _launch(ops, probs)
-        for p in probs:
-            out[p.c.name] = p.y.cpu().numpy()
-            out[p.c.name + "_st"] = p.st.cpu().numpy()
-    elif which == "ksplit":
-        p = Prob(ops, _KS_CASE)
-        _launch(ops, [p])
-        out["y"] = p.y.cpu().numpy()
-        out["ksplit"] = np.array(ops.conv1d_fused_last_config()["ksplit"])
-    else:                                               # a dependent chain of split-K launches (6 output tiles, 4 K chunks)
-        t = _inputs(_PDL_CHAIN)
-        cw = ops.pack_conv(t["w"], t["bias"], 1, DEV)
-        y = t["x"].to(DEV)
-        for _ in range(8):
-            y = ops.conv_fused(ops.FusedProblem(y, cw, pad_left=1, post_act=ACT["tanh"]))[0]
-        out["ksplit"] = np.array(ops.conv1d_fused_last_config()["ksplit"])
-        torch.cuda.synchronize()
-        out["y"] = y.cpu().numpy()
+    t = _inputs(_PDL_CHAIN)
+    cw = ops.pack_conv(t["w"], t["bias"], 1, DEV)
+    y = t["x"].to(DEV)
+    for _ in range(8):
+        y = ops.conv_fused(ops.FusedProblem(y, cw, pad_left=1, post_act=ACT["tanh"]))[0]
+    out["ksplit"] = np.array(ops.conv1d_fused_last_config()["ksplit"])
+    torch.cuda.synchronize()
+    out["y"] = y.cpu().numpy()
     return out
 
 
-def _switch_child(which: str, path: str):
-    np.savez(path, **_scenario(which))
+def _switch_child(path: str):
+    np.savez(path, **_pdl_chain())
 
 
-def _run_child(which, env, tmp_path):
-    path = str(tmp_path / f"{which}.npz")
+def _run_child(env, tmp_path):
+    path = str(tmp_path / "pdl.npz")
     code = (f"import sys; sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'tests')!r}]\n"
-            f"import test_conv_fused_matrix_gpu as m\nm._switch_child({which!r}, {path!r})\n")
+            f"import test_conv_fused_matrix_gpu as m\nm._switch_child({path!r})\n")
     subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), check=True, timeout=600)
     return dict(np.load(path))
 
 
-def test_interleave_switch_identical(ops, tmp_path):
-    """B2A_FUSED_INTERLEAVE=1 on three problems with equal tile counts, Cin <= 320 and their own statistics prologues: the interleaved
-    tile order (one coefficient table per problem) gives the default order's bits."""
-    plan = _plan(_IL_GROUP, _nsm(), ops.FUSED_WS_BYTES)
-    assert plan.ksplit == [1, 1, 1] and len({-(-c.mrows // TM) * (c.N // c.bn) * c.B for c in _IL_GROUP}) == 1, plan
-    default = _scenario("interleave")
-    for c in _IL_GROUP:
-        p = Prob(ops, c)
-        _launch(ops, [p])
-        p.check()
-    child = _run_child("interleave", {"B2A_FUSED_INTERLEAVE": "1"}, tmp_path)
-    assert set(child) == set(default)
-    for k in default:
-        assert np.array_equal(child[k], default[k]), k
-
-
-def test_ksplit_switch_off(ops, tmp_path):
-    """B2A_FUSED_KSPLIT=0: a layer that splits K by default runs unsplit and stays within tolerance."""
-    default = _scenario("ksplit")
-    assert default["ksplit"][0] > 1
-    child = _run_child("ksplit", {"B2A_FUSED_KSPLIT": "0"}, tmp_path)
-    assert list(child["ksplit"]) == [1]
-    ref = _reference(_KS_CASE, _inputs(_KS_CASE), Prob(ops, _KS_CASE).stats_val)
-    assert rel_err(torch.from_numpy(child["y"]), ref) <= TOL_X2
-    assert rel_err(torch.from_numpy(default["y"]), ref) <= TOL_X2
-
-
 def test_pdl_switch_off_identical(ops, tmp_path):
     """B2A_FUSED_PDL=0: a dependent chain launched without programmatic dependent launch gives the same bits."""
-    default = _scenario("pdl")
-    child = _run_child("pdl", {"B2A_FUSED_PDL": "0"}, tmp_path)
+    default = _pdl_chain()
+    child = _run_child({"B2A_FUSED_PDL": "0"}, tmp_path)
     assert default["ksplit"][0] > 1 and np.isfinite(default["y"]).all()
     assert np.array_equal(child["y"], default["y"])
 

@@ -1,4 +1,4 @@
-"""Compile-time guard for the continuous-batching kernels: the four attention / cache kernels that take per-row cache positions and a
+"""Compile-time guard for the continuous-batching kernels: the three attention / cache kernels that take per-row cache positions and a
 slot map (lm.cu, attn_prefill.cu) and the slot-advance kernel build for sm_90a with the library's flags, and ptxas reports no spills."""
 import os
 import re
@@ -8,7 +8,7 @@ import pytest
 
 from mlx_audio_b200 import build
 
-KERNELS = {"lm.cu": ["qknorm_rope_cache_kernel", "attn_decode_kernel", "attn_decode_fused_kernel", "slot_advance_kernel"],
+KERNELS = {"lm.cu": ["qknorm_rope_cache_kernel", "attn_decode_kernel", "slot_advance_kernel"],
            "attn_prefill.cu": ["attn_prefill_kernel"]}
 
 

@@ -126,38 +126,3 @@ def test_convtr1d_tc_polyphase(B, L, Cin, Cout, K, stride, pad, opad, path):
     finally:
         ops.TC_MODE[0] = old
     assert y.shape == ref.shape and rel_err(y, ref) < 2e-5
-
-
-@pytest.mark.parametrize("L,Cin,Cout,K,transpose,stride", [(390, 256, 128, 3, False, 1), (7801, 128, 256, 7, False, 1), (300, 128, 64, 16, True, 8),
-                                                           (130, 64, 96, 1, False, 1)])
-def test_epilogue_instance_norm_partials(L, Cin, Cout, K, transpose, stride):
-    """conv1d(stats=True): conv_tc_kernel's epilogue emits InstanceNorm partial sums of its output; the AdaIN coefficients
-    built from them equal the ones from the separate statistics pass (istftnet.py:216-268) -- ragged last tile, residual,
-    up-sampling phases included."""
-    from mlx_audio_b200 import ops
-    dev = torch.device("cuda:0")
-    x = _rand(2, L, Cin, seed=1)
-    w = _rand(Cout, K, Cin, seed=2, scale=0.05).to(torch.bfloat16).float()
-    cw = ops.pack_conv(w, _rand(Cout, seed=3, scale=0.1), 1, dev)
-    gb = _rand(2, 2 * Cout, seed=4, scale=0.3).to(dev)
-    old, ops.TC_STATS[0] = ops.TC_STATS[0], True          # opt-in feature (off by default: measured slower end to end)
-    oldf, ops.FUSED[0] = ops.FUSED[0], False              # this is gemm_tc.cu's epilogue; the fused kernel's statistics: test_fused_gpu.py
-    try:
-        _run_stats_case(ops, dev, x, cw, gb, L, Cout, K, transpose, stride)
-    finally:
-        ops.TC_STATS[0], ops.FUSED[0] = old, oldf
-
-
-def _run_stats_case(ops, dev, x, cw, gb, L, Cout, K, transpose, stride):
-    if transpose:
-        y, part = ops.conv1d(x.to(dev), cw, stride=stride, pad_left=(K - stride) // 2, transpose=True, stats=True)
-    else:
-        res = _rand(2, L, Cout, seed=5).to(dev)
-        y, part = ops.conv1d(x.to(dev), cw, pad_left=(K - 1) // 2, res=res, out_scale=0.7, stats=True)
-    assert part is not None and part.dtype == torch.float64
-    s_ref, h_ref = ops.adain_coeffs(y, gb)
-    s_got, h_got = ops.adain_coeffs(y, gb, partials=part)
-    assert rel_err(s_got, s_ref) < 1e-5 and rel_err(h_got, h_ref) < 1e-5
-    mean = y.double().mean(dim=1)
-    got_mean = part[..., 0].sum(dim=1) / y.shape[1]
-    assert float((got_mean - mean).abs().max()) < 1e-6

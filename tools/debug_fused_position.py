@@ -27,7 +27,6 @@ check("C128 k7 L1000 slice 200:800 bf16-exact w", 128, 128, 7, 1, 1000, 200, 800
 check("C512 k3 L300 slice 50:250", 512, 256, 3, 1, 300, 50, 250)
 check("C128 k1 L20000 slice 5000:15000", 128, 128, 1, 1, 20000, 5000, 15000)
 check("C128 k7 L40000 slice 5000:35000 (no split-K either way)", 128, 128, 7, 1, 40000, 5000, 35000)
-os.environ["B2A_FUSED_KSPLIT"] = "1"
 
 print("--- through ops.conv1d (dispatcher), SNAC-shaped layers")
 from mlx_audio_b200.ops import Pre, ACT
