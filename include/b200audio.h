@@ -97,6 +97,12 @@ enum {
 };
 int32_t b2a_conv1d_cl_last_path(int32_t* out4);
 
+/* Kokoro's harmonic-source convs (istftnet.py noise_convs) on har [B, L, 22] (contiguous): (K, stride) = (12, 6) or (1, 1), Cout a
+ * multiple of 128, weights packed [K][22][Cout] as for b2a_conv1d_cl, zero padding, bias then y [B, Lout, Cout] (contiguous).
+ * Bit-identical to b2a_conv1d_cl on the same layer (x 8-byte, w and y 16-byte aligned). */
+int32_t b2a_kokoro_source_conv(const float* x, int32_t B, int32_t L, const float* w, const float* bias, float* y, int32_t Lout,
+                               int32_t Cout, int32_t K, int32_t stride, int32_t pad_left, void* stream);
+
 /* ---- tensor-core path for dense stride-1 convs / Linears (csrc/gemm_tc.cu) --------------------------------
  * b2a_prep_bf16: the conv prologue (pre_scale/shift + activation, as in b2a_conv1d_t) evaluated once per element and
  * stored as two bf16 planes hi = bf16(v), lo = bf16(v - hi), each [B, L, cpad] (cpad multiple of 64, pad channels zero);

@@ -91,6 +91,7 @@ PROTOTYPES = {
     "b2a_conv1d_cl": (i32, [C.POINTER(Conv1dParams), C.c_void_p]),
     "b2a_convtr1d_cl": (i32, [C.POINTER(Conv1dParams), C.c_void_p]),
     "b2a_conv1d_cl_last_path": (i32, [C.POINTER(i32)]),
+    "b2a_kokoro_source_conv": (i32, [c_f, i32, i32, c_f, c_f, c_f, i32, i32, i32, i32, i32, C.c_void_p]),
     "b2a_prep_bf16": (i32, [c_f, i64, i64, i32, i32, i32, i32, c_f, c_f, i32, f32, c_f, c_f, c_f, c_f, i32, C.c_void_p]),
     "b2a_conv1d_tc": (i32, [c_f, c_f, i32, i32, i32, i32, c_f, c_f, i32, C.POINTER(i32), i32, i32, c_f, i32, f32, c_f, i64, c_f, i64, i64, i32, f32, i32,
                             c_f, i64, i64, i32, i32, c_f, c_f, i64, c_f, i32, f32, C.c_void_p]),

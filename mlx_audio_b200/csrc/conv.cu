@@ -723,6 +723,129 @@ extern "C" int32_t b2a_convtr1d_cl(const b2a_conv1d_t* p, void* stream) {
   return B2A_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Kokoro's harmonic-source convs (istftnet.py:780-800 noise_convs): 22 input channels (the source STFT's magnitude | phase),
+// (K, stride) = (12, 6) into 256 channels and (1, 1) into 128.  The generic dense tile pads the 22 channels to its chunk width and
+// pays runtime divisions for every staged element; here Cin, K and the stride are compile-time constants.  A CTA owns
+// SC_BM positions x SC_BN channels: its input span is ONE contiguous block of rows x 22 floats (staged with 8-byte loads, zero
+// outside [0, L)) and its weight slice [K][22][SC_BN] is staged once.  Warp = 64 positions x 32 channels; lane (tm, tn) owns
+// positions tm + 8i (i < 8: consecutive lanes read rows stride*22 floats apart, distinct banks) and channels tn*8 .. tn*8+7.
+//
+// Every output gets exactly the fmaf sequence of conv1d_dense_kernel, whose chunk width is CI = 16 for K = 12 and 32 for K = 1:
+// chunks [0, SPLIT) then [SPLIT, 22), each taps ascending then channels ascending, then bias.  The dense tile's zero-padded
+// channels 22 .. CI-1 run fmaf(0, 0, acc) after each tap of the last chunk; that equals acc + 0 (identity except -0 -> +0), and a
+// run of them equals one, so each is replaced by a single add of +0.
+namespace {
+constexpr int SC_CIN = 22, SC_BM = 128, SC_BN = 128;
+
+template <int K, int S>
+__global__ void __launch_bounds__(NT, 2) kokoro_source_conv_kernel(const float* __restrict__ x, int L, const float* __restrict__ w,
+                                                                   const float* __restrict__ bias, float* __restrict__ y, int Lout,
+                                                                   int Cout, int pad_left) {
+  constexpr int SPLIT = K == 1 ? SC_CIN : 16;                  // channel chunks of the dense tile: CI = 32 (K <= 4) or 16 (K <= 12)
+  constexpr int ROWS = (SC_BM - 1) * S + K;
+  constexpr int XS = ((ROWS * SC_CIN + 3) / 4) * 4;             // floats of the staged input span, 16-byte aligned end
+  extern __shared__ __align__(16) float smem[];
+  float* xs = smem;                                             // [ROWS][22]
+  float* ws = smem + XS;                                        // [K][22][SC_BN]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tn = lane & 3, tm = lane >> 2;
+  const int wn = warp & 3, wm = warp >> 2;
+  const int l0 = blockIdx.x * SC_BM, n0 = blockIdx.y * SC_BN, b = blockIdx.z;
+  const int64_t e0 = ((int64_t)l0 * S - pad_left) * SC_CIN;     // first staged element (even: 22 is)
+  const int64_t ne = (int64_t)L * SC_CIN;
+  const float* xb = x + (int64_t)b * ne;
+  for (int e = 2 * tid; e < ROWS * SC_CIN; e += 2 * NT) {
+    const int64_t g = e0 + e;
+    float2 v = make_float2(0.f, 0.f);
+    if (g >= 0 && g < ne) v = __ldg(reinterpret_cast<const float2*>(xb + g));
+    *reinterpret_cast<float2*>(xs + e) = v;
+  }
+  for (int e = 4 * tid; e < K * SC_CIN * SC_BN; e += 4 * NT) {
+    const int r = e / SC_BN, n = e - r * SC_BN;
+    *reinterpret_cast<float4*>(ws + e) = __ldg(reinterpret_cast<const float4*>(w + (int64_t)r * Cout + n0 + n));
+  }
+  __syncthreads();
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; i++)
+#pragma unroll
+    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
+  const float* xr = xs + (wm * 64 + tm) * S * SC_CIN;
+  const float* wr = ws + wn * 32 + tn * 8;
+  auto step = [&](int k, int c) {
+    float a[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) a[i] = xr[(8 * i * S + k) * SC_CIN + c];
+    const float4 w0 = *reinterpret_cast<const float4*>(wr + (k * SC_CIN + c) * SC_BN);
+    const float4 w1 = *reinterpret_cast<const float4*>(wr + (k * SC_CIN + c) * SC_BN + 4);
+    const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+#pragma unroll
+      for (int j = 0; j < 8; j++) acc[i][j] = fmaf(a[i], wv[j], acc[i][j]);
+  };
+  if constexpr (SPLIT < SC_CIN) {
+#pragma unroll 1
+    for (int k = 0; k < K; k++) {
+#pragma unroll
+      for (int c = 0; c < SPLIT; c++) step(k, c);
+    }
+  }
+#pragma unroll 1
+  for (int k = 0; k < K; k++) {
+#pragma unroll
+    for (int c = SPLIT < SC_CIN ? SPLIT : 0; c < SC_CIN; c++) step(k, c);
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+#pragma unroll
+      for (int j = 0; j < 8; j++) acc[i][j] = __fadd_rn(acc[i][j], 0.f);     // the padded channels' fmaf(0, 0, acc)
+  }
+  const int co = n0 + wn * 32 + tn * 8;
+  float bv[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) bv[j] = bias ? __ldg(bias + co + j) : 0.f;
+  float* yb = y + (int64_t)b * Lout * Cout + co;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    const int l = l0 + wm * 64 + tm + 8 * i;
+    if (l >= Lout) break;
+    float o[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) o[j] = bias ? acc[i][j] + bv[j] : acc[i][j];
+    *reinterpret_cast<float4*>(yb + (int64_t)l * Cout) = make_float4(o[0], o[1], o[2], o[3]);
+    *reinterpret_cast<float4*>(yb + (int64_t)l * Cout + 4) = make_float4(o[4], o[5], o[6], o[7]);
+  }
+}
+
+template <int K, int S>
+int32_t launch_kokoro_source_conv(const float* x, int32_t B, int32_t L, const float* w, const float* bias, float* y, int32_t Lout,
+                                  int32_t Cout, int32_t pad_left, cudaStream_t st) {
+  constexpr int ROWS = (SC_BM - 1) * S + K;
+  const size_t sm = ((size_t)((ROWS * SC_CIN + 3) / 4) * 4 + (size_t)K * SC_CIN * SC_BN) * sizeof(float);
+  static bool attr = false;
+  if (!attr) { cudaFuncSetAttribute(kokoro_source_conv_kernel<K, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); attr = true; }
+  dim3 grid(cdiv(Lout, SC_BM), Cout / SC_BN, B);
+  kokoro_source_conv_kernel<K, S><<<grid, NT, sm, st>>>(x, L, w, bias, y, Lout, Cout, pad_left);
+  B2A_CHECK_LAUNCH();
+  return B2A_OK;
+}
+}  // namespace
+
+/* Kokoro's noise_convs on the harmonic source har [B, L, 22] (contiguous) -> y [B, Lout, Cout] (contiguous); bit-identical to
+ * b2a_conv1d_cl on the same layer */
+extern "C" int32_t b2a_kokoro_source_conv(const float* x, int32_t B, int32_t L, const float* w, const float* bias, float* y, int32_t Lout,
+                                          int32_t Cout, int32_t K, int32_t stride, int32_t pad_left, void* stream) {
+  B2A_CHECK_ARG(x && w && y && B > 0 && L > 0 && Lout > 0, "bad pointers / shape");
+  B2A_CHECK_ARG(Cout > 0 && Cout % SC_BN == 0, "Cout must be a multiple of 128");
+  B2A_CHECK_ARG(((uintptr_t)x & 7) == 0 && ((uintptr_t)w & 15) == 0 && ((uintptr_t)y & 15) == 0, "x needs 8-byte, w and y 16-byte alignment");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (K == 12 && stride == 6) return launch_kokoro_source_conv<12, 6>(x, B, L, w, bias, y, Lout, Cout, pad_left, st);
+  if (K == 1 && stride == 1) return launch_kokoro_source_conv<1, 1>(x, B, L, w, bias, y, Lout, Cout, pad_left, st);
+  b2a_set_error("b2a_kokoro_source_conv: (K, stride) must be (12, 6) or (1, 1), got (%d, %d)", K, stride);
+  return B2A_E_UNSUPPORTED;
+}
+
 extern "C" int32_t b2a_copy2d(const float* src, int64_t src_ld, float* dst, int64_t dst_ld, int64_t rows, int32_t cols, void* stream) {
   B2A_CHECK_ARG(src && dst && rows >= 0 && cols > 0, "bad pointers/shape");
   if (rows == 0) return B2A_OK;

@@ -1000,6 +1000,22 @@ def kokoro_source(f0: torch.Tensor, noise: Optional[torch.Tensor], lin_w: torch.
     return har
 
 
+def kokoro_source_conv(har: torch.Tensor, cw: ConvW, *, stride: int = 1, pad_left: int = 0) -> torch.Tensor:
+    """A noise conv on the harmonic source: har [B, L, 22] -> [B, Lout, Cout], bit-identical to ``conv1d(har, cw, stride=, pad_left=)``
+    (csrc/conv.cu, b2a_kokoro_source_conv: (K, stride) = (12, 6) or (1, 1))."""
+    _chk3(har, "kokoro_source_conv har")
+    B, L, cin = har.shape
+    if cin != 22 or cw.cin != 22 or cw.groups != 1 or not har.is_contiguous():
+        raise ValueError("kokoro_source_conv: expected a contiguous [B, L, 22] source and a dense 22-channel layer")
+    lout = (L + 2 * pad_left - cw.K) // stride + 1
+    out = torch.empty(B, lout, cw.cout, device=har.device, dtype=torch.float32)
+    if PROFILE_TAGS is not None:
+        TAG[0] = f"source conv [{B}x{L}x{cin}->{cw.cout} k{cw.K} s{stride}]"
+    _call("conv" if cin * cw.K >= 64 else "other", _lib.lib().b2a_kokoro_source_conv, 1, har.data_ptr(), B, L, cw.w.data_ptr(), _p(cw.bias),
+          out.data_ptr(), lout, cw.cout, cw.K, stride, pad_left, _stream())
+    return out
+
+
 def kokoro_istft_head(x: torch.Tensor) -> torch.Tensor:
     """conv_post output [B,T,22] -> waveform [B, (T-1)*5]."""
     _chk3(x, "kokoro_istft_head x")

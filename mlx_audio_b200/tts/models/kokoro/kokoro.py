@@ -444,18 +444,22 @@ class Model:
         def source_branch():
             har = ops.kokoro_source(f0_curve.reshape(1, 2 * F), noise, *W["src_lin"])      # [1,120F+1,22]
             self._tap("har", har)
+            ts = []
             for i in range(len(rates)):
                 if i + 1 < len(rates):
                     sf0 = math.prod(rates[i + 1:])
-                    t = ops.conv1d(har, W["noise_convs"][i], stride=sf0, pad_left=(sf0 + 1) // 2)
+                    t = ops.kokoro_source_conv(har, W["noise_convs"][i], stride=sf0, pad_left=(sf0 + 1) // 2)
                 else:
-                    t = ops.conv1d(har, W["noise_convs"][i])
+                    t = ops.kokoro_source_conv(har, W["noise_convs"][i])
                 ops.channel_stats(t, src_stats[i])
-                pool, self._stats_pool = self._stats_pool, list(src_arena[i])
-                try:
-                    self._resblock1_group([t], [src_stats[i]], [W["noise_res"][i]], outs=[xsrcs[i]])
-                finally:
-                    self._stats_pool = pool
+                ts.append(t)
+            # both noise-resblock chains in shared launches (one problem per up-sampling stage); _resblock1_group takes a statistics
+            # buffer for each problem in turn, so the reserved buffers are interleaved by stage
+            pool, self._stats_pool = self._stats_pool, [s for group in zip(*src_arena) for s in group]
+            try:
+                self._resblock1_group(ts, src_stats, W["noise_res"], outs=xsrcs)
+            finally:
+                self._stats_pool = pool
 
         if par:
             side_src = ops.fork(dev, 1)
