@@ -1057,9 +1057,10 @@ def sample_token(logits: torch.Tensor, *, temperature: float, top_k: int = 0, to
 
 
 def gemv_eligible(cw: "ConvW") -> bool:
-    """The decode GEMV streams ONE bf16 plane of weights: bf16-exact K=1 layers only (fp16 / fp32 checkpoints and layers whose
-    Cout is not a multiple of 32 go through ``linear``)."""
-    return cw.K == 1 and cw.w_tc is not None and not cw.f16 and cw.w_tc_lo is None
+    """The decode GEMV streams ONE bf16 plane of weights in 16-byte (8-element) loads: bf16-exact K=1 layers whose input width is a
+    multiple of 8 only (fp16 / fp32 checkpoints, layers whose Cout is not a multiple of 32 and other input widths go through
+    ``linear``)."""
+    return cw.K == 1 and cw.w_tc is not None and not cw.f16 and cw.w_tc_lo is None and cw.cin % 8 == 0
 
 
 def gemv(x: torch.Tensor, cw: "ConvW", *, norm_w=None, norm_eps: float = 1e-6, swiglu: bool = False, res=None, out=None,
@@ -1068,7 +1069,8 @@ def gemv(x: torch.Tensor, cw: "ConvW", *, norm_w=None, norm_eps: float = 1e-6, s
     optional fused RMSNorm prologue, SwiGLU (interleaved gate/up rows) and residual.  ``prefetch``: the next projection, whose
     weights are pulled into L2 while this one runs."""
     if not (x.dim() == 2 and x.stride(1) == 1 and gemv_eligible(cw)):
-        raise NotImplementedError("gemv needs a bf16-exact K=1 weight with Cout % 32 == 0 (see ops.gemv_eligible); use ops.linear")
+        raise NotImplementedError("gemv needs a bf16-exact K=1 weight with Cout % 32 == 0 and Cin % 8 == 0 (see ops.gemv_eligible); "
+                                  "use ops.linear")
     M, K = x.shape
     N = cw.cout
     n_out = N // 2 if swiglu else N

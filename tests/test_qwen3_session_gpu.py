@@ -25,31 +25,13 @@ def rel_err(a, b):
 
 
 # ------------------------------------------------------------------------------------------------------------------- kernels
-def _attn_ref(q, kc, vc, Hq, Hkv, D, base_rows, slot, scale):
-    """float64 causal GQA attention: query s of row b sees rows [0, base_rows[b] + s] of cache batch slot[b]; negative positions -> 0."""
-    B, S, _ = q.shape
-    G = Hq // Hkv
-    out = torch.zeros(B, S, Hq * D, dtype=torch.float64)
-    for b in range(B):
-        for s in range(S):
-            pos = int(base_rows[b]) + s
-            if pos < 0:
-                continue
-            k = kc[int(slot[b]), : pos + 1].double().view(pos + 1, Hkv, D)
-            v = vc[int(slot[b]), : pos + 1].double().view(pos + 1, Hkv, D)
-            qh = q[b, s].double().view(Hq, D)
-            for h in range(Hq):
-                p = torch.softmax((k[:, h // G] @ qh[h]) * scale, dim=0)
-                out[b, s, h * D:(h + 1) * D] = p @ v[:, h // G]
-    return out
-
-
 @pytest.mark.parametrize("D,Hq,Hkv,S", [(128, 16, 8, 1), (64, 4, 2, 1), (128, 4, 2, 5), (128, 4, 2, 96)], ids=["decode-d128", "decode-d64", "S5", "prefill-S96"])
 def test_ragged_cache_kernels(D, Hq, Hkv, S):
     """qknorm_rope_cache + attn_decode / attn_prefill with ragged ``base_rows`` (one of them negative: a
     left-padding row) and a slot map with gaps, against float64 attention; padding positions write nothing and read zero; each
     kernel's output is bit-identical to the scalar-base path run on the same rows one at a time."""
     from mlx_audio_b200 import ops
+    from test_lm_decode_matrix_gpu import cache_attn_ref   # tests/ is on sys.path (rootdir-relative "prepend" import mode)
     dev = _dev()
     g = torch.Generator().manual_seed(D + S)
     nslots, rows = 5, 320
@@ -75,7 +57,7 @@ def test_ragged_cache_kernels(D, Hq, Hkv, S):
         assert torch.equal(qb[0], q[b, first:]), b
     assert torch.equal(kr, kc) and torch.equal(vr, vc)         # identical rows written, nothing for padding, other slots untouched
     scale = D ** -0.5
-    want = _attn_ref(q.cpu(), kc.cpu(), vc.cpu(), Hq, Hkv, D, base_rows, slot, scale)
+    want = cache_attn_ref(q.cpu(), kc.cpu(), vc.cpu(), Hq, Hkv, D, base_rows, slot, None, rows, scale)
     attn = ops.attn_prefill if S >= 64 else ops.attn_decode
     if S >= 64 and (D != 128 or Hq != 2 * Hkv):
         pytest.skip("prefill kernel shape")
