@@ -205,7 +205,8 @@ int32_t b2a_layernorm(const float* x, int64_t x_ld, const float* res, int64_t re
  * softmax(scale * q k^T + mask) v with fp32 softmax; replaces mx.fast.scaled_dot_product_attention
  * (mimi/modules/transformer.py:109, talker.py:307) and the unfused form (whisper.py:371-385, modules.py:497-505).
  * q [B,Tq,H,D], k/v [B,Tk,Hkv,D] with token strides *_ld and batch strides *_bs (elements); head h at +h*D.
- * causal != 0: key j visible to query i iff j <= i + q_offset; window > 0: also i + q_offset - j < window. */
+ * causal != 0: key j visible to query i iff j <= i + q_offset; window > 0 (only with causal != 0, else an invalid argument): also
+ * i + q_offset - j < window.  q, k, v, o 16-byte aligned, all strides multiples of 4. */
 typedef struct {
   const float* q; const float* k; const float* v; float* o;
   int64_t q_bs, q_ld, k_bs, k_ld, v_bs, v_ld, o_bs, o_ld;
@@ -220,7 +221,12 @@ int32_t b2a_attention(const b2a_attn_t* p, void* stream);
 /* Same contract on the tensor cores (wgmma) for D == 64, H == Hkv, k_len == NULL: S = QK^T and PV as fp16 hi/lo-plane MMAs
  * (fp32-grade products), online softmax with one thread per query row.  ws: device scratch of b2a_attention_tc_ws_bytes bytes
  * (fp16 planes of q * scale * log2(e), k and the transposed v, keys zero-padded to a multiple of 8).  Launched with programmatic
- * dependent launch. */
+ * dependent launch.
+ * Operand envelope: the result is fp32-grade (within 2e-5 of float64) while the operands stay above ~2^-10 in magnitude and
+ * q * scale * log2(e), k and v stay below fp16's 65504.  fp16's subnormal floor (2^-24) limits the lo planes, which matters for v
+ * (it scales the output): v of rms 2^-6 .. 2^8 measured within 2e-6 on an H100 80GB HBM3 (700 W); v of rms 2^-10 is emulated at
+ * 1.4e-5; v of rms 1e-4 measured 1.4e-4, as a float64 emulation of the split predicts.  Small q or k only shrink the scores.
+ * tests/test_attention_norm_matrix_gpu.py pins these numbers. */
 int64_t b2a_attention_tc_ws_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk);
 int32_t b2a_attention_tc(const b2a_attn_t* p, void* ws, void* stream);
 /* in-place rotary embedding on x [B,T,H,D] (token stride ld): traditional != 0 rotates pairs (2i,2i+1)

@@ -128,7 +128,10 @@ __global__ void rope_kernel(float* __restrict__ x, int64_t x_bs, int64_t x_ld, i
 extern "C" int32_t b2a_attention(const b2a_attn_t* p, void* stream) {
   B2A_CHECK_ARG(p && p->q && p->k && p->v && p->o, "null pointer");
   B2A_CHECK_ARG(p->B > 0 && p->Tq > 0 && p->Tk > 0 && p->H > 0 && p->Hkv > 0 && p->H % p->Hkv == 0, "bad shape");
+  B2A_CHECK_ARG(p->window <= 0 || p->causal, "a sliding window needs causal masking");
   B2A_CHECK_ARG((p->q_ld % 4 == 0) && (p->k_ld % 4 == 0) && (p->v_ld % 4 == 0) && (p->o_ld % 4 == 0), "token strides must be multiples of 4");
+  B2A_CHECK_ARG((p->q_bs % 4 == 0) && (p->k_bs % 4 == 0) && (p->v_bs % 4 == 0) && (p->o_bs % 4 == 0), "batch strides must be multiples of 4");
+  B2A_CHECK_ARG((((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->o) & 15) == 0, "q/k/v/o must be 16-byte aligned");
   dim3 grid(cdiv(p->Tq, QT), p->H, p->B);
   if (p->D == 64) attn_kernel<64><<<grid, QT, 0, (cudaStream_t)stream>>>(*p);
   else { b2a_set_error("b2a_attention: head dim %d not supported (64)", p->D); return B2A_E_UNSUPPORTED; }

@@ -211,6 +211,7 @@ extern "C" int32_t b2a_attention_tc(const b2a_attn_t* a, void* ws, void* stream)
   B2A_CHECK_ARG(a && ws && a->o && (a->operands_ready || (a->q && a->k && a->v)), "null pointer");
   B2A_CHECK_ARG(a->D == 64 && a->H == a->Hkv && a->k_len == nullptr, "tensor-core attention: head_dim 64, no GQA, no per-row key length");
   B2A_CHECK_ARG(a->B > 0 && a->Tq > 0 && a->Tk > 0 && a->H > 0, "bad shape");
+  B2A_CHECK_ARG(a->window <= 0 || a->causal, "a sliding window needs causal masking");
   B2A_CHECK_ARG(a->operands_ready ||
                 (a->q_ld % 4 == 0 && a->k_ld % 4 == 0 && a->q_bs % 4 == 0 && a->k_bs % 4 == 0 && ((uintptr_t)a->q & 15) == 0 && ((uintptr_t)a->k & 15) == 0),
                 "q/k rows must be 16-byte aligned");

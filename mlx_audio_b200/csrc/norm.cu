@@ -182,8 +182,9 @@ extern "C" int32_t b2a_layernorm(const float* x, int64_t x_ld, const float* res,
                                  int64_t rows, int32_t C, const float* w, const float* b, const float* ada, float eps,
                                  int32_t rms, int32_t post_act, float post_p0, void* emit_hi, void* emit_lo, int64_t emit_ld,
                                  void* stream) {
-  B2A_CHECK_ARG(x && y && rows >= 0 && C > 0, "bad pointers/shape");
-  if (rows == 0) return B2A_OK;
+  B2A_CHECK_ARG(rows >= 0 && C > 0, "bad shape");
+  if (rows == 0) return B2A_OK;                            // before the pointer check: an empty torch tensor has a null data pointer
+  B2A_CHECK_ARG(x && y, "null pointer");
   const bool al = C % 4 == 0 && C <= 1024 && x_ld % 4 == 0 && y_ld % 4 == 0 && (!res || res_ld % 4 == 0) && ((uintptr_t)x & 15) == 0 &&
                   ((uintptr_t)y & 15) == 0 && (!res || ((uintptr_t)res & 15) == 0);
   B2A_CHECK_ARG(!emit_hi || (al && emit_ld >= C && emit_ld % 4 == 0 && ((uintptr_t)emit_hi & 7) == 0 && ((uintptr_t)emit_lo & 7) == 0),

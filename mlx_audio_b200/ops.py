@@ -831,9 +831,12 @@ def layernorm(x: torch.Tensor, w=None, b=None, *, eps=1e-5, res=None, ada=None, 
 
 
 def attention(q, k, v, *, n_heads, n_kv_heads=None, scale, causal=False, q_offset=0, window=0, k_len=None, out=None):
-    """softmax(scale q k^T + mask) v.  q [B,Tq,H*D], k/v [B,Tk,Hkv*D] (row-strided views allowed)."""
+    """softmax(scale q k^T + mask) v.  q [B,Tq,H*D], k/v [B,Tk,Hkv*D] (row-strided views allowed).  ``window`` > 0 limits the causal
+    mask to the last ``window`` positions, so it needs ``causal=True``."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _chk3(t, "attention " + n)
+    if window > 0 and not causal:
+        raise ValueError(f"attention: a sliding window ({window}) needs causal=True")
     B, Tq, hd = q.shape
     H = n_heads
     Hkv = n_kv_heads or H
