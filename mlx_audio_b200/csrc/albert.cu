@@ -332,28 +332,6 @@ __global__ void __launch_bounds__(THREADS, 1) albert_kernel(const __grid_constan
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_enc = nullptr;
-
-// 16-bit tensor of `rank` (2 or 3) dims, innermost first; box 64 x 64 (x 1), 128B swizzle
-int map16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, bool f16) {
-  if (!g_enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) return -1;
-    g_enc = (EncodeTiledFn)fn;
-  }
-  cuuint64_t gd[3]; cuuint64_t gs[2]; cuuint32_t bx[3] = {64, 64, 1}; cuuint32_t es[3] = {1, 1, 1};
-  for (int i = 0; i < rank; i++) gd[i] = dims[i];
-  for (int i = 0; i < rank - 1; i++) gs[i] = strides_bytes[i];
-  CUresult r = g_enc(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd,
-                     gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
 // workspace: barrier counter | t | u (fp32 [T][hs]) | cp, ap (bf16 hi, lo [T][hs]) | fp (bf16 hi, lo [T][inter]) | attention operands
 struct WsLayout { int64_t t, u, cp_hi, cp_lo, ap_hi, ap_lo, fp_hi, fp_lo, attn, total; };
 WsLayout ws_layout(int64_t T, int64_t H, int64_t hs, int64_t inter) {
@@ -410,37 +388,30 @@ extern "C" int32_t b2a_albert_encoder(const b2a_albert_t* a, void* ws, uint32_t*
   AlbertMaps m;
   const void* a_hi[4] = {p.hp_hi, p.cp_hi, p.ap_hi, p.fp_hi};
   const void* a_lo[4] = {p.hp_lo, p.cp_lo, p.ap_lo, p.fp_lo};
+  const uint32_t box[3] = {64, 64, 1};              // every operand map: 64 x 64 (x 1) tiles
   int e = 0;
   for (int i = 0; i < 4 && !e; i++) {
     const uint64_t ad[2] = {(uint64_t)K[i], (uint64_t)T}, as[1] = {(uint64_t)K[i] * 2};
     const uint64_t wd[2] = {(uint64_t)K[i], (uint64_t)N[i]};
-    e = map16(&m.a_hi[i], a_hi[i], 2, ad, as, false);
-    if (!e) e = map16(&m.a_lo[i], a->planes == 2 ? a_lo[i] : a_hi[i], 2, ad, as, false);
-    if (!e) e = map16(&m.w[i], a->w[i], 2, wd, as, false);
+    e = b2a_tmap16(&m.a_hi[i], a_hi[i], 2, ad, as, box, false);
+    if (!e) e = b2a_tmap16(&m.a_lo[i], a->planes == 2 ? a_lo[i] : a_hi[i], 2, ad, as, box, false);
+    if (!e) e = b2a_tmap16(&m.w[i], a->w[i], 2, wd, as, box, false);
   }
   const uint64_t qd[3] = {64, (uint64_t)T, (uint64_t)H}, qs[2] = {128, (uint64_t)T * 128};
   const uint64_t vd[3] = {(uint64_t)p.attn.tkp, 64, (uint64_t)H}, vs[2] = {(uint64_t)p.attn.tkp * 2, (uint64_t)p.attn.tkp * 128};
-  if (!e) e = map16(&m.qh, p.attn.qh, 3, qd, qs, true);
-  if (!e) e = map16(&m.ql, p.attn.ql, 3, qd, qs, true);
-  if (!e) e = map16(&m.kh, p.attn.kh, 3, qd, qs, true);
-  if (!e) e = map16(&m.kl, p.attn.kl, 3, qd, qs, true);
-  if (!e) e = map16(&m.vh, p.attn.vh, 3, vd, vs, true);
-  if (!e) e = map16(&m.vl, p.attn.vl, 3, vd, vs, true);
+  if (!e) e = b2a_tmap16(&m.qh, p.attn.qh, 3, qd, qs, box, true);
+  if (!e) e = b2a_tmap16(&m.ql, p.attn.ql, 3, qd, qs, box, true);
+  if (!e) e = b2a_tmap16(&m.kh, p.attn.kh, 3, qd, qs, box, true);
+  if (!e) e = b2a_tmap16(&m.kl, p.attn.kl, 3, qd, qs, box, true);
+  if (!e) e = b2a_tmap16(&m.vh, p.attn.vh, 3, vd, vs, box, true);
+  if (!e) e = b2a_tmap16(&m.vl, p.attn.vl, 3, vd, vs, box, true);
   if (e) { b2a_set_error("b2a_albert_encoder: cuTensorMapEncodeTiled failed (%d)", e); return B2A_E_CUDA; }
 
   void (*kern)(const AlbertMaps, const AlbertParams) = timeline ? albert_kernel<true> : albert_kernel<false>;
-  static bool attr[2] = {false, false};
-  if (!attr[timeline ? 1 : 0]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
-      b2a_set_error("b2a_albert_encoder: cannot raise the dynamic shared-memory limit: %s", cudaGetErrorString(cudaGetLastError()));
-      return B2A_E_CUDA;
-    }
-    attr[timeline ? 1 : 0] = true;
-  }
+  B2A_SMEM_OPTIN(kern, SMEM_BYTES);
   // one CTA per SM, as many as can be co-resident (the cooperative launch refuses a grid that cannot)
-  int dev = 0, nsm = 0, per_sm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  const int nsm = b2a_device_sm_count();
+  int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, SMEM_BYTES) != cudaSuccess || per_sm < 1 || nsm < 1) {
     b2a_set_error("b2a_albert_encoder: the kernel cannot be resident (%s)", cudaGetErrorString(cudaGetLastError()));
     return B2A_E_CUDA;

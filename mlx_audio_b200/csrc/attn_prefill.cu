@@ -252,8 +252,7 @@ extern "C" int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, 
   B2A_CHECK_ARG(o_ss % 2 == 0 && o_bs % 2 == 0 && ((uintptr_t)out & 7) == 0, "out rows must be 8-byte aligned");
   PfParams p{q, q_bs, q_ss, k_cache, v_cache, c_bs, c_ss, out, o_bs, o_ss, S, Hkv, scale * 1.4426950408889634f,
              base_dev, base_host, kv_start, max_k, base_rows, slot};
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(attn_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); attr = true; }
+  B2A_SMEM_OPTIN(attn_prefill_kernel, SMEM_BYTES);
   dim3 grid((unsigned)((S + BM - 1) / BM), (unsigned)Hkv, (unsigned)B);
   b2a_launch_pdl(attn_prefill_kernel, grid, dim3(THREADS), SMEM_BYTES, (cudaStream_t)stream, p);
   B2A_CHECK_LAUNCH();

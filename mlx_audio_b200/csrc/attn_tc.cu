@@ -182,24 +182,6 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_enc = nullptr;
-
-int map3(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1, uint64_t s2, uint32_t b0, uint32_t b1) {
-  if (!g_enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) return -1;
-    g_enc = (EncodeTiledFn)fn;
-  }
-  cuuint64_t gd[3] = {d0, d1, d2}; cuuint64_t gs[2] = {s1, s2}; cuuint32_t bx[3] = {b0, b1, 1}; cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = g_enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
 }  // namespace
 
 extern "C" int64_t b2a_attention_tc_ws_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk) {
@@ -233,17 +215,20 @@ extern "C" int32_t b2a_attention_tc(const b2a_attn_t* a, void* ws, void* stream)
     attn_tc_prep_vt_kernel<<<gv, 256, 0, st>>>(a->v, a->v_bs, a->v_ld, B, H, Tk, (int)Tkp, vh, vl);
   }
   CUtensorMap mqh, mql, mkh, mkl, mvh, mvl;
-  int e = map3(&mqh, qh, HD, Tq, bh, HD * 2, (uint64_t)Tq * HD * 2, HD, BM);
-  if (!e) e = map3(&mql, ql, HD, Tq, bh, HD * 2, (uint64_t)Tq * HD * 2, HD, BM);
-  if (!e) e = map3(&mkh, kh, HD, Tk, bh, HD * 2, (uint64_t)Tk * HD * 2, HD, BN);
-  if (!e) e = map3(&mkl, kl, HD, Tk, bh, HD * 2, (uint64_t)Tk * HD * 2, HD, BN);
-  if (!e) e = map3(&mvh, vh, Tkp, HD, bh, Tkp * 2, (uint64_t)HD * Tkp * 2, BN, HD);
-  if (!e) e = map3(&mvl, vl, Tkp, HD, bh, Tkp * 2, (uint64_t)HD * Tkp * 2, BN, HD);
+  const uint64_t qd[3] = {HD, (uint64_t)Tq, (uint64_t)bh}, qs[2] = {HD * 2, (uint64_t)Tq * HD * 2};
+  const uint64_t kd[3] = {HD, (uint64_t)Tk, (uint64_t)bh}, ks[2] = {HD * 2, (uint64_t)Tk * HD * 2};
+  const uint64_t vd[3] = {(uint64_t)Tkp, HD, (uint64_t)bh}, vs[2] = {(uint64_t)Tkp * 2, (uint64_t)HD * Tkp * 2};
+  const uint32_t qb[3] = {HD, BM, 1}, kb[3] = {HD, BN, 1}, vb[3] = {BN, HD, 1};
+  int e = b2a_tmap16(&mqh, qh, 3, qd, qs, qb, true);
+  if (!e) e = b2a_tmap16(&mql, ql, 3, qd, qs, qb, true);
+  if (!e) e = b2a_tmap16(&mkh, kh, 3, kd, ks, kb, true);
+  if (!e) e = b2a_tmap16(&mkl, kl, 3, kd, ks, kb, true);
+  if (!e) e = b2a_tmap16(&mvh, vh, 3, vd, vs, vb, true);
+  if (!e) e = b2a_tmap16(&mvl, vl, 3, vd, vs, vb, true);
   if (e) { b2a_set_error("b2a_attention_tc: cuTensorMapEncodeTiled failed (%d)", e); return B2A_E_CUDA; }
   AtcParams p{B, H, Tq, Tk, a->causal, a->q_offset, a->window, a->o, a->o_bs, a->o_ld,
               (__nv_bfloat16*)a->emit_hi, (__nv_bfloat16*)a->emit_lo, a->emit_ld};
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); attr = true; }
+  B2A_SMEM_OPTIN(attn_tc_kernel, SMEM_BYTES);
   dim3 grid((Tq + BM - 1) / BM, (unsigned)bh);
   if (b2a_launch_pdl(attn_tc_kernel, grid, dim3(THREADS), SMEM_BYTES, st, mqh, mql, mkh, mkl, mvh, mvl, p) != cudaSuccess) {
     b2a_set_error("b2a_attention_tc: %s", cudaGetErrorString(cudaGetLastError()));

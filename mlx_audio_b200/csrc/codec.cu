@@ -197,8 +197,7 @@ extern "C" int32_t b2a_rvq_encode(const float* x, int64_t x_ld, int64_t rows, in
                 "bad pointers / shape (dim % 4 == 0; mode 1 = one level)");
   const size_t smem = (size_t)VQ_ROWS * dim * 8 + VQ_ROWS * 8 * 8 + VQ_ROWS * 8 * 4;
   B2A_CHECK_ARG(smem <= 200 * 1024, "dim too large");
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(rvq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
+  B2A_SMEM_OPTIN(rvq_encode_kernel, 200 * 1024);
   rvq_encode_kernel<<<(unsigned)((rows + VQ_ROWS - 1) / VQ_ROWS), 256, smem, (cudaStream_t)stream>>>(x, x_ld, rows, dim, codebooks, c2, bins, nq, mode, codes,
                                                                                                     codes_row_stride, codes_level_stride);
   B2A_CHECK_LAUNCH();

@@ -15,6 +15,17 @@ void b2a_set_error(const char* fmt, ...);
   do { cudaError_t e_ = cudaGetLastError();                        \
        if (e_ != cudaSuccess) { b2a_set_error("%s: %s", __func__, cudaGetErrorString(e_)); return B2A_E_CUDA; } } while (0)
 
+// Raise `kernel`'s dynamic shared-memory limit to at least `bytes` (api.cu).  Thread-safe; a limit never goes down, and the runtime is
+// called only when it has to grow, so launch paths call this before every launch.
+cudaError_t b2a_smem_optin(const void* kernel, int bytes);
+
+// The same, returning B2A_E_CUDA from the calling function when the opt-in fails.  A template id with a comma goes in parentheses.
+#define B2A_SMEM_OPTIN(kernel, bytes)                                                                                         \
+  do { cudaError_t e_ = b2a_smem_optin((const void*)(kernel), (int)(bytes));                                                   \
+       if (e_ != cudaSuccess) {                                                                                                 \
+         b2a_set_error("%s: cannot raise the dynamic shared-memory limit to %d bytes: %s", __func__, (int)(bytes), cudaGetErrorString(e_)); \
+         return B2A_E_CUDA; } } while (0)
+
 // sin for the Snake activations: two-constant Cody-Waite reduction to [-pi, pi] + the SFU sine (abs error < 5e-7 there), ~6
 // instructions instead of libm's ~40 -- the prologue kernels that apply Snake are otherwise instruction-bound, not HBM-bound.
 __device__ __forceinline__ float b2a_sin(float x) {

@@ -593,25 +593,17 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
       ((size_t)(NW_TL + (p->K - 1) * p->dilation) * (p->Cin + 1) + (size_t)p->K * p->Cin * p->Cout) * sizeof(float) <= 160 * 1024) {
     const int rows = NW_TL + (p->K - 1) * p->dilation;
     const size_t sm = ((size_t)rows * (p->Cin + 1) + (size_t)p->K * p->Cin * p->Cout) * sizeof(float);
-    static bool attr = false;
-    if (!attr) {
-      cudaFuncSetAttribute(conv1d_narrow_kernel<-1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-      cudaFuncSetAttribute(conv1d_narrow_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-      cudaFuncSetAttribute(conv1d_narrow_kernel<B2A_ACT_SNAKE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-      cudaFuncSetAttribute(conv1d_narrow_kernel<B2A_ACT_ELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-      cudaFuncSetAttribute(conv1d_narrow_kernel<B2A_ACT_LRELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-      attr = true;
-    }
     dim3 grid(cdiv(p->Lout, NW_TL), p->B);
     const bool v4 = (p->Cin % 4 == 0) && (p->x_ld % 4 == 0) && (p->x_bs % 4 == 0) && (((uintptr_t)p->x & 15) == 0);
     const int act = p->pre_scale ? -1
                   : (p->pre_act == 0 || p->pre_act == B2A_ACT_ELU || p->pre_act == B2A_ACT_LRELU ||
                      (p->pre_act == B2A_ACT_SNAKE && p->pre_a && p->pre_b)) ? p->pre_act : -1;
-    if (act == 0) conv1d_narrow_kernel<0><<<grid, NT, sm, st>>>(*p, rows, v4);
-    else if (act == B2A_ACT_SNAKE) conv1d_narrow_kernel<B2A_ACT_SNAKE><<<grid, NT, sm, st>>>(*p, rows, v4);
-    else if (act == B2A_ACT_ELU) conv1d_narrow_kernel<B2A_ACT_ELU><<<grid, NT, sm, st>>>(*p, rows, v4);
-    else if (act == B2A_ACT_LRELU) conv1d_narrow_kernel<B2A_ACT_LRELU><<<grid, NT, sm, st>>>(*p, rows, v4);
-    else conv1d_narrow_kernel<-1><<<grid, NT, sm, st>>>(*p, rows, v4);
+    const auto kern = act == 0 ? conv1d_narrow_kernel<0>
+                    : act == B2A_ACT_SNAKE ? conv1d_narrow_kernel<B2A_ACT_SNAKE>
+                    : act == B2A_ACT_ELU ? conv1d_narrow_kernel<B2A_ACT_ELU>
+                    : act == B2A_ACT_LRELU ? conv1d_narrow_kernel<B2A_ACT_LRELU> : conv1d_narrow_kernel<-1>;
+    B2A_SMEM_OPTIN(kern, 160 * 1024);
+    kern<<<grid, NT, sm, st>>>(*p, rows, v4);
     kernel = B2A_CONV_PATH_NARROW; v1 = act; v3 = v4;
   } else if (p->groups == 1) {
     const int CI = p->K <= 4 ? 32 : (p->K <= 12 ? 16 : 8);
@@ -620,15 +612,9 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
     size_t smem = ((((size_t)rows * (CI + 1) + 3) & ~(size_t)3) + (size_t)p->K * CI * BN) * sizeof(float);
     if (smem > 200 * 1024) { b2a_set_error("b2a_conv1d_cl: tile needs %zu B of shared memory", smem); return B2A_E_UNSUPPORTED; }
     dim3 grid(cdiv(p->Lout, BM), cdiv(p->Cout, BN), p->B);
-    if (BN == 64) {
-      static bool attr = false;
-      if (!attr) { cudaFuncSetAttribute(conv1d_dense_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
-      conv1d_dense_kernel<64><<<grid, NT, smem, st>>>(*p, CI, rows);
-    } else {
-      static bool attr = false;
-      if (!attr) { cudaFuncSetAttribute(conv1d_dense_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
-      conv1d_dense_kernel<16><<<grid, NT, smem, st>>>(*p, CI, rows);
-    }
+    const auto kern = BN == 64 ? conv1d_dense_kernel<64> : conv1d_dense_kernel<16>;
+    B2A_SMEM_OPTIN(kern, 200 * 1024);
+    kern<<<grid, NT, smem, st>>>(*p, CI, rows);
     kernel = B2A_CONV_PATH_DENSE; v1 = BN; v2 = CI;
   } else if (p->groups == p->Cin && p->Cin == p->Cout) {
     int rows = DW_TL + (p->K - 1) * p->dilation;
@@ -645,37 +631,18 @@ extern "C" int32_t b2a_conv1d_cl(const b2a_conv1d_t* p, void* stream) {
       dim3 grid((p->Lout + DW_TL - 1) / DW_TL, (p->Cout + CW - 1) / CW, p->B);
       const size_t sm = (size_t)rows * CW * sizeof(float);
       const bool snake = p->pre_act == B2A_ACT_SNAKE && !p->pre_scale && (!p->emit_hi || p->emit_act == B2A_ACT_SNAKE);
-      static bool attr = false;
-      if (!attr) {
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<7, 128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<7, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<7, 128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<7, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<0, 128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        cudaFuncSetAttribute(conv1d_dw_tiled4_kernel<0, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        attr = true;
-      }
-      if (p->K == 7 && snake && (p->emit_hi || true)) {
-        if (CW == 128) conv1d_dw_tiled4_kernel<7, 128, true><<<grid, NT, sm, st>>>(*p, rows);
-        else conv1d_dw_tiled4_kernel<7, 64, true><<<grid, NT, sm, st>>>(*p, rows);
-      } else if (p->K == 7) {
-        if (CW == 128) conv1d_dw_tiled4_kernel<7, 128, false><<<grid, NT, sm, st>>>(*p, rows);
-        else conv1d_dw_tiled4_kernel<7, 64, false><<<grid, NT, sm, st>>>(*p, rows);
-      } else {
-        if (CW == 128) conv1d_dw_tiled4_kernel<0, 128, false><<<grid, NT, sm, st>>>(*p, rows);
-        else conv1d_dw_tiled4_kernel<0, 64, false><<<grid, NT, sm, st>>>(*p, rows);
-      }
+      const auto kern = p->K == 7 && snake ? (CW == 128 ? conv1d_dw_tiled4_kernel<7, 128, true> : conv1d_dw_tiled4_kernel<7, 64, true>)
+                      : p->K == 7 ? (CW == 128 ? conv1d_dw_tiled4_kernel<7, 128, false> : conv1d_dw_tiled4_kernel<7, 64, false>)
+                      : (CW == 128 ? conv1d_dw_tiled4_kernel<0, 128, false> : conv1d_dw_tiled4_kernel<0, 64, false>);
+      B2A_SMEM_OPTIN(kern, 160 * 1024);
+      kern<<<grid, NT, sm, st>>>(*p, rows);
       kernel = B2A_CONV_PATH_DW_TILED4; v1 = CW; v2 = p->K == 7 ? 7 : 0; v3 = p->K == 7 && snake;
     } else if (p->stride == 1 && p->K <= 16 && rows * 32 * 4 <= 96 * 1024 && p->Lout >= DW_TL) {
       dim3 grid((p->Lout + DW_TL - 1) / DW_TL, (p->Cout + 31) / 32, p->B);
       size_t sm = (size_t)rows * 32 * sizeof(float);
-      if (p->K == 7) {
-        if (sm > 48 * 1024) cudaFuncSetAttribute(conv1d_dw_tiled_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        conv1d_dw_tiled_kernel<7><<<grid, NT, sm, st>>>(*p, rows);
-      } else {
-        if (sm > 48 * 1024) cudaFuncSetAttribute(conv1d_dw_tiled_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        conv1d_dw_tiled_kernel<0><<<grid, NT, sm, st>>>(*p, rows);
-      }
+      const auto kern = p->K == 7 ? conv1d_dw_tiled_kernel<7> : conv1d_dw_tiled_kernel<0>;
+      B2A_SMEM_OPTIN(kern, 96 * 1024);
+      kern<<<grid, NT, sm, st>>>(*p, rows);
       kernel = B2A_CONV_PATH_DW_TILED; v1 = p->K == 7 ? 7 : 0;
     } else {
       int64_t total = (int64_t)p->B * p->Lout * p->Cout;
@@ -705,8 +672,7 @@ extern "C" int32_t b2a_convtr1d_cl(const b2a_conv1d_t* p, void* stream) {
     const int rows = (BM - 1) / p->stride + J + 1;
     size_t smem = ((((size_t)rows * (CI + 1) + 3) & ~(size_t)3) + (size_t)p->K * CI * 64) * sizeof(float);
     if (smem > 200 * 1024) { b2a_set_error("b2a_convtr1d_cl: tile needs %zu B of shared memory", smem); return B2A_E_UNSUPPORTED; }
-    static bool attr = false;
-    if (!attr) { cudaFuncSetAttribute(convtr1d_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
+    B2A_SMEM_OPTIN(convtr1d_dense_kernel, 200 * 1024);
     dim3 grid(cdiv(p->Lout, BM), cdiv(p->Cout, 64), p->B);
     convtr1d_dense_kernel<<<grid, NT, smem, st>>>(*p, CI, rows, J);
     B2A_CHECK_LAUNCH();
@@ -823,8 +789,7 @@ int32_t launch_kokoro_source_conv(const float* x, int32_t B, int32_t L, const fl
                                   int32_t Cout, int32_t pad_left, cudaStream_t st) {
   constexpr int ROWS = (SC_BM - 1) * S + K;
   const size_t sm = ((size_t)((ROWS * SC_CIN + 3) / 4) * 4 + (size_t)K * SC_CIN * SC_BN) * sizeof(float);
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(kokoro_source_conv_kernel<K, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); attr = true; }
+  B2A_SMEM_OPTIN((kokoro_source_conv_kernel<K, S>), sm);
   dim3 grid(cdiv(Lout, SC_BM), Cout / SC_BN, B);
   kokoro_source_conv_kernel<K, S><<<grid, NT, sm, st>>>(x, L, w, bias, y, Lout, Cout, pad_left);
   B2A_CHECK_LAUNCH();

@@ -707,21 +707,8 @@ conv_fused_kernel(const __grid_constant__ FParams gp, const __grid_constant__ CU
     p.dbg[(size_t)blockIdx.x * 32 + 26 + threadIdx.x] = mwait_all[threadIdx.x] + mwait_all[MW_N + threadIdx.x];
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_enc = nullptr;
 unsigned long long* g_fdbg = nullptr;
 thread_local int32_t g_last_cfg[2 + 2 * MAXG] = {};    // problems, grid, then (BN, ksplit) per problem: this host thread's last launch
-
-int get_enc() {
-  if (g_enc) return 0;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) return -1;
-  g_enc = (EncodeTiledFn)fn;
-  return 0;
-}
 
 // N tile: the widest divisor of N (multiple of 32, <= 128) -- in polyphase mode also a divisor of C so that a tile stays inside one phase
 int n_tile(int N, int C) {
@@ -747,16 +734,6 @@ int weight_stages(int a_plane, int planes, int acc_ld, int w_stage, size_t* smem
   return wst;
 }
 
-int make_wmap(CUtensorMap* m, const void* base, uint64_t cin_pad, uint64_t rows, uint32_t bn, int f16) {
-  cuuint64_t gd[2] = {cin_pad, rows};
-  cuuint64_t gs[1] = {cin_pad * 2};
-  cuuint32_t bx[2] = {TK, bn};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = g_enc(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gd, gs, bx, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
 }  // namespace
 
 /* debug aid: device buffer of [gridDim][32] uint64 that the next launches stamp with %globaltimer at their phase boundaries (NULL: off) */
@@ -778,13 +755,7 @@ extern "C" int32_t b2a_conv1d_fused_fits(int32_t span, int32_t N, int32_t C, int
 
 extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t planes, int32_t f16, void* ws, int64_t ws_bytes, void* stream) {
   B2A_CHECK_ARG(pr && n >= 1 && n <= MAXG && (planes == 1 || planes == 2), "1..4 problems, planes 1 or 2");
-  if (get_enc() != 0) { b2a_set_error("b2a_conv1d_fused: cuTensorMapEncodeTiled entry point not found"); return B2A_E_CUDA; }
-  static int nsm = 0, pdl = -1;
-  if (!nsm) {
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-    if (nsm <= 0) nsm = 132;
-    const char* e = getenv("B2A_FUSED_PDL"); pdl = (e && e[0] == '0') ? 0 : 1;
-  }
+  static const int nsm = [] { const int n = b2a_device_sm_count(); return n > 0 ? n : 132; }();
   FParams p;
   p.G = n; p.planes = planes; p.f16 = f16 ? 1 : 0; p.dbg = g_fdbg;
   { static int flags = -1; if (flags < 0) { const char* e = getenv("B2A_FUSED_DBGFLAGS"); flags = e ? atoi(e) : 0; } p.dbg_flags = flags; }
@@ -874,30 +845,18 @@ extern "C" int32_t b2a_conv1d_fused(const b2a_convf_t* pr, int32_t n, int32_t pl
   for (int gi = 0; gi < MAXG; gi++) {
     const b2a_convf_t& q = pr[order[gi < n ? gi : 0]];
     const FProb& P = p.pr[gi < n ? gi : 0];
-    int e = make_wmap(&mw[gi], q.w_hi, (uint64_t)q.cin_pad, (uint64_t)q.taps * q.N, (uint32_t)P.BN, p.f16);
-    if (!e) e = make_wmap(&ml[gi], q.w_lo ? q.w_lo : q.w_hi, (uint64_t)q.cin_pad, (uint64_t)q.taps * q.N, (uint32_t)P.BN, p.f16);
+    const uint64_t wdims[2] = {(uint64_t)q.cin_pad, (uint64_t)q.taps * q.N}, wstr[1] = {(uint64_t)q.cin_pad * 2};
+    const uint32_t wbox[2] = {TK, (uint32_t)P.BN};
+    int e = b2a_tmap16(&mw[gi], q.w_hi, 2, wdims, wstr, wbox, p.f16);
+    if (!e) e = b2a_tmap16(&ml[gi], q.w_lo ? q.w_lo : q.w_hi, 2, wdims, wstr, wbox, p.f16);
     if (e) { b2a_set_error("b2a_conv1d_fused: cuTensorMapEncodeTiled failed (%d)", e); return B2A_E_CUDA; }
   }
-  static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(conv_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DYN_SMEM_MAX) != cudaSuccess ||
-        cudaFuncSetAttribute(conv_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DYN_SMEM_MAX) != cudaSuccess) {
-      cudaGetLastError();
-      b2a_set_error("b2a_conv1d_fused: cannot raise the dynamic shared-memory limit to %d bytes", (int)DYN_SMEM_MAX);
-      return B2A_E_CUDA;
-    }
-    attr = true;
-  }
-  const int grid = tiles_total < nsm ? tiles_total : nsm;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-  cfg.attrs = at; cfg.numAttrs = 1;
   const bool dbg = p.dbg != nullptr || p.dbg_flags != 0;
-  cudaError_t err = dbg ? cudaLaunchKernelEx(&cfg, conv_fused_kernel<true>, p, mw[0], mw[1], mw[2], mw[3], ml[0], ml[1], ml[2], ml[3])
-                        : cudaLaunchKernelEx(&cfg, conv_fused_kernel<false>, p, mw[0], mw[1], mw[2], mw[3], ml[0], ml[1], ml[2], ml[3]);
+  const auto kern = dbg ? conv_fused_kernel<true> : conv_fused_kernel<false>;
+  B2A_SMEM_OPTIN(kern, DYN_SMEM_MAX);
+  const int grid = tiles_total < nsm ? tiles_total : nsm;
+  cudaError_t err = b2a_launch_pdl(kern, dim3(grid), dim3(THREADS), smem, (cudaStream_t)stream, p, mw[0], mw[1], mw[2], mw[3], ml[0], ml[1],
+                                   ml[2], ml[3]);
   if (err != cudaSuccess) { b2a_set_error("b2a_conv1d_fused: launch failed: %s", cudaGetErrorString(err)); return B2A_E_CUDA; }
   B2A_CHECK_LAUNCH();
   for (int i = 0; i < 2 + 2 * MAXG; i++) g_last_cfg[i] = 0;

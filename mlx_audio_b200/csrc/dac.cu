@@ -203,8 +203,7 @@ extern "C" int32_t b2a_dac_rvq_encode(const float* z, int64_t z_ld, int32_t B, i
   B2A_CHECK_ARG(latent_channels >= n_levels && latent_channels <= n_levels * DQ_MAX_CD, "codebook_dim must be in [1, 16] at every level");
   const size_t smem = (size_t)b2a_dac_rvq_encode_smem_bytes(dim);
   B2A_CHECK_ARG(smem <= 160 * 1024, "latent dimension too large for the frame tile");
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(dac_rvq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024); attr = true; }
+  B2A_SMEM_OPTIN(dac_rvq_encode_kernel, 160 * 1024);
   const int64_t R = (int64_t)B * T;
   dac_rvq_encode_kernel<<<(unsigned)((R + DQ_FRAMES - 1) / DQ_FRAMES), DQ_THREADS, smem, (cudaStream_t)stream>>>(
       z, z_ld, R, T, dim, levels_dev, n_levels, bins, latent_channels, codes, latents, z_q, loss_part);

@@ -307,8 +307,7 @@ extern "C" int32_t b2a_stft(const float* x, int64_t x_bs, int32_t B, int64_t n, 
   B2A_CHECK_ARG(n_fft >= 2 && n_fft <= 4096 && n_fft % 2 == 0, "n_fft must be even and <= 4096");
   if (pad_mode == 1) B2A_CHECK_ARG(n > n_fft / 2, "reflect padding needs n > n_fft/2");
   size_t smem = (size_t)(2 + FT) * n_fft * sizeof(float);
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
+  B2A_SMEM_OPTIN(stft_kernel, 200 * 1024);
   dim3 grid(cdiv(frames, FT), B);
   stft_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(x, x_bs, n, window, n_fft, hop, pad_mode, frames, out_re, out_im);
   B2A_CHECK_LAUNCH();
@@ -322,8 +321,7 @@ extern "C" int32_t b2a_whisper_logmel(const float* x, int64_t x_bs, int32_t B, i
   cudaStream_t st = (cudaStream_t)stream;
   cudaMemsetAsync(gmax, 0, sizeof(float) * B, st);
   size_t smem = (size_t)((2 + FT) * 400 + FT * 201) * sizeof(float);
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(whisper_logmel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024); attr = true; }
+  B2A_SMEM_OPTIN(whisper_logmel_kernel, 64 * 1024);
   dim3 grid(cdiv(frames, FT), B);
   whisper_logmel_kernel<<<grid, 256, smem, st>>>(x, x_bs, n, padding, window, filters, n_mels, frames, out, gmax);
   int64_t per = frames * n_mels;
@@ -339,8 +337,7 @@ extern "C" int32_t b2a_istft(const float* re, const float* im, int32_t B, int32_
   cudaStream_t st = (cudaStream_t)stream;
   size_t smem = (size_t)(2 * n_fft + 2 * (n_fft / 2 + 1)) * sizeof(float);
   dim3 grid(T, B);
-  static bool attr = false;      // n_fft = 4096 needs 49 160 B of dynamic shared memory, just above the 48 KB default
-  if (!attr) { cudaFuncSetAttribute(irfft_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024); attr = true; }
+  B2A_SMEM_OPTIN(irfft_frames_kernel, 64 * 1024);      // n_fft = 4096 needs 49 160 B of dynamic shared memory, just above the 48 KB default
   irfft_frames_kernel<<<grid, 128, smem, st>>>(re, im, n_fft, T, window, ws);
   ola_kernel<<<grid_for(out_len * B, 256), 256, 0, st>>>(ws, n_fft, T, hop, window, norm_sq, clamp_mode, trim, out_len, out, B);
   B2A_CHECK_LAUNCH();

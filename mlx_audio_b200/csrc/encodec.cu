@@ -210,7 +210,7 @@ int32_t launch_lstm(const float* xproj, const float* wh, const float* skip, floa
   auto kern = encodec_lstm_kernel<H, RB>;
   const size_t smem = lstm_smem_bytes<H>(RB);
   constexpr int NCTA = LstmGeom<H>::NCTA;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = b2a_smem_optin((const void*)kern, (int)smem);
   if (e == cudaSuccess && NCTA > 8) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
   if (e != cudaSuccess) { b2a_set_error("b2a_encodec_lstm: %s", cudaGetErrorString(e)); return B2A_E_CUDA; }
   cudaLaunchConfig_t cfg = {};

@@ -300,31 +300,8 @@ __global__ void prep_bf16_kernel(const float* __restrict__ x, int64_t x_bs, int6
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
 long long* g_dbg = nullptr;
 thread_local int32_t g_last_cfg[5] = {0, 0, 0, 0, 0};   // BN, grid x / y / z, stages of this host thread's last launch
-
-int get_encode() {
-  if (g_encode) return 0;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) return -1;
-  g_encode = (EncodeTiledFn)fn;
-  return 0;
-}
-
-int make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int f16) {
-  cuuint64_t gd[3]; cuuint64_t gs[2]; cuuint32_t bx[3]; cuuint32_t es[3] = {1, 1, 1};
-  for (int i = 0; i < rank; i++) { gd[i] = dims[i]; bx[i] = box[i]; }
-  for (int i = 0; i < rank - 1; i++) gs[i] = strides_bytes[i];
-  CUresult r = g_encode(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
 
 }  // namespace
 
@@ -374,7 +351,6 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
                 "transposed mode: Cout = up_stride * C with C a multiple of 32");
   B2A_CHECK_ARG(B > 0 && L > 0 && Lout > 0 && taps > 0 && taps <= 32 && cin_pad % 64 == 0 && (res_div == 1 || res_div == 2), "bad shape (res_div must be 1 or 2)");
   B2A_CHECK_ARG(Cout % 32 == 0 && y_ld % 4 == 0 && (res == nullptr || res_ld % 4 == 0), "Cout must be a multiple of 32; row strides multiples of 4");
-  if (get_encode() != 0) { b2a_set_error("b2a_conv1d_tc: cuTensorMapEncodeTiled entry point not found"); return B2A_E_CUDA; }
   TcParams p;
   p.f16 = f16 ? 1 : 0;
   p.wplanes = w_lo ? 2 : 1;
@@ -390,8 +366,7 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
   // Few-row GEMMs (ALBERT at T = 130: 2 row tiles) leave most SMs idle at that width and every CTA runs the whole K loop alone:
   // when the grid covers under half the SMs, take the widest tile whose grid still reaches the SM count, else the narrowest (32).
   // Each output element still accumulates its whole K range in the same order inside one CTA.
-  static int nsm = 0;
-  if (!nsm) { nsm = b2a_device_sm_count(); if (nsm <= 0) nsm = 132; }
+  static const int nsm = [] { const int n = b2a_device_sm_count(); return n > 0 ? n : 132; }();
   const int64_t row_tiles = (int64_t)cdiv(p.Mrows, TM) * B;
   if (row_tiles * (Cout / p.BN) * 2 < nsm) {
     int bn = 32;
@@ -418,32 +393,23 @@ extern "C" int32_t b2a_conv1d_tc(const void* a_hi, const void* a_lo, int32_t f16
   uint64_t adims[3] = {(uint64_t)cin_pad, (uint64_t)L, (uint64_t)B};
   uint64_t astr[2] = {(uint64_t)cin_pad * 2, (uint64_t)cin_pad * 2 * (uint64_t)L};
   uint32_t abox[3] = {TK, TM, 1};
-  int e = make_map(&mh, a_hi, 3, adims, astr, abox, p.f16);
-  if (!e) e = make_map(&ml, a_lo ? a_lo : a_hi, 3, adims, astr, abox, p.f16);
+  int e = b2a_tmap16(&mh, a_hi, 3, adims, astr, abox, p.f16);
+  if (!e) e = b2a_tmap16(&ml, a_lo ? a_lo : a_hi, 3, adims, astr, abox, p.f16);
   uint64_t wdims[2] = {(uint64_t)cin_pad, (uint64_t)taps * Cout};
   uint64_t wstr[1] = {(uint64_t)cin_pad * 2};
   uint32_t wbox[2] = {TK, (uint32_t)p.BN};
-  if (!e) e = make_map(&mw, w_bf16, 2, wdims, wstr, wbox, p.f16);
-  if (!e) e = make_map(&mwl, w_lo ? w_lo : w_bf16, 2, wdims, wstr, wbox, p.f16);
+  if (!e) e = b2a_tmap16(&mw, w_bf16, 2, wdims, wstr, wbox, p.f16);
+  if (!e) e = b2a_tmap16(&mwl, w_lo ? w_lo : w_bf16, 2, wdims, wstr, wbox, p.f16);
   if (e) { b2a_set_error("b2a_conv1d_tc: cuTensorMapEncodeTiled failed (%d)", e); return B2A_E_CUDA; }
 
   typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcParams);
   static const KernelFn kernels[2][4] = {
       {conv_tc_kernel<1, false>, conv_tc_kernel<2, false>, conv_tc_kernel<3, false>, conv_tc_kernel<4, false>},
       {conv_tc_kernel<1, true>, conv_tc_kernel<2, true>, conv_tc_kernel<3, true>, conv_tc_kernel<4, true>}};
-  static bool attr = false;
-  if (!attr) {
-    for (int i = 0; i < 2; i++)
-      for (int j = 0; j < 4; j++)
-        if (cudaFuncSetAttribute(kernels[i][j], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-          cudaGetLastError();
-          b2a_set_error("b2a_conv1d_tc: cannot raise the dynamic shared-memory limit");
-          return B2A_E_CUDA;
-        }
-    attr = true;
-  }
+  const KernelFn kern = kernels[p.f16][p.BN / 32 - 1];
+  B2A_SMEM_OPTIN(kern, 227 * 1024);
   dim3 grid(cdiv(p.Mrows, TM), Cout / p.BN, B);
-  if (b2a_launch_pdl(kernels[p.f16][p.BN / 32 - 1], grid, dim3(THREADS), smem, (cudaStream_t)stream, mh, ml, mw, mwl, p) != cudaSuccess) {
+  if (b2a_launch_pdl(kern, grid, dim3(THREADS), smem, (cudaStream_t)stream, mh, ml, mw, mwl, p) != cudaSuccess) {
     b2a_set_error("b2a_conv1d_tc: %s", cudaGetErrorString(cudaGetLastError()));
     return B2A_E_CUDA;
   }

@@ -441,16 +441,6 @@ __global__ void __launch_bounds__(AD_THREADS) attn_decode_kernel(const AdParams 
   }
 }
 
-// Without the opt-in a CTA's static shared memory (redm / reds and what the toolchain adds) and the dynamic score buffer share 48 KB,
-// so the dynamic limit is below 48 KB: it is read from the function, and a launch that needs more opts in first.
-template <int D>
-void launch_attn_decode(dim3 grid, size_t sm, cudaStream_t st, const AdParams& p) {
-  cudaFuncAttributes fa;
-  if (cudaFuncGetAttributes(&fa, attn_decode_kernel<D>) == cudaSuccess && sm > (size_t)fa.maxDynamicSharedSizeBytes)
-    cudaFuncSetAttribute(attn_decode_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-  b2a_launch_pdl(attn_decode_kernel<D>, grid, dim3(AD_THREADS), sm, st, p);
-}
-
 __global__ void swiglu_kernel(const float* x, int64_t x_ld, int64_t rows, int I, int interleaved, float* y, int64_t y_ld) {
   const int64_t total = rows * I;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -579,10 +569,9 @@ extern "C" int32_t b2a_attn_decode(const float* q, int64_t q_bs, int64_t q_ss, c
   if (floats < (size_t)(AD_THREADS / 32) * D) floats = (size_t)(AD_THREADS / 32) * D;
   const size_t sm = floats * sizeof(float);
   dim3 grid(Hq, S, B);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (D == 128) launch_attn_decode<128>(grid, sm, st, p);
-  else if (D == 64) launch_attn_decode<64>(grid, sm, st, p);
-  else launch_attn_decode<32>(grid, sm, st, p);
+  const auto kern = D == 128 ? attn_decode_kernel<128> : D == 64 ? attn_decode_kernel<64> : attn_decode_kernel<32>;
+  B2A_SMEM_OPTIN(kern, sm);
+  b2a_launch_pdl(kern, grid, dim3(AD_THREADS), sm, (cudaStream_t)stream, p);
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }

@@ -258,12 +258,7 @@ extern "C" int32_t b2a_lm_sample_mlx(const float* logits, int64_t logits_bs, int
   p.finished = finished; p.stop0 = stop0; p.stop1 = stop1;
   p.cache = V <= LS_CACHE_MAX;
   const size_t smem = (size_t)LS_BINS * LS_THREADS * sizeof(double) + (p.cache ? (size_t)V * sizeof(float) : 0);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(lm_sample_mlx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)(LS_BINS * LS_THREADS * sizeof(double) + LS_CACHE_MAX * sizeof(float)));
-    attr_set = true;
-  }
+  B2A_SMEM_OPTIN(lm_sample_mlx_kernel, LS_BINS * LS_THREADS * sizeof(double) + LS_CACHE_MAX * sizeof(float));
   lm_sample_mlx_kernel<<<B, LS_THREADS, smem, (cudaStream_t)stream>>>(p);
   B2A_CHECK_LAUNCH();
   return B2A_OK;

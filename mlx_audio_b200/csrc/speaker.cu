@@ -314,8 +314,7 @@ extern "C" int32_t b2a_spk_logmel(const float* x, int64_t x_bs, int32_t B, int64
   B2A_CHECK_ARG(n > MEL_PAD, "reflect padding needs more than 384 samples");
   B2A_CHECK_ARG(frames == 1 + (n + 2 * MEL_PAD - MEL_N) / MEL_HOP, "frames must be 1 + (n + 768 - 1024) / 256");
   const size_t smem = spk_logmel_smem_bytes();
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(spk_logmel_kernel<MEL_PAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+  B2A_SMEM_OPTIN((spk_logmel_kernel<MEL_PAD, true>), smem);
   dim3 grid(cdiv(frames, MEL_FT), B);
   spk_logmel_kernel<MEL_PAD, true><<<grid, 256, smem, (cudaStream_t)stream>>>(x, x_bs, n, window, filters, n_mels, frames, out);
   B2A_CHECK_LAUNCH();
@@ -351,13 +350,9 @@ extern "C" int32_t b2a_spk_res2net(const float* y, int64_t y_bs, int64_t y_ld, f
   if (smem > 227 * 1024) { b2a_set_error("%s: %lld bytes of shared memory", __func__, (long long)smem); return B2A_E_UNSUPPORTED; }
   dim3 grid(cdiv(T, tile), B);
   cudaStream_t st = (cudaStream_t)stream;
-  if (C % 4 == 0) {
-    cudaFuncSetAttribute(spk_res2net_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    spk_res2net_kernel<4><<<grid, 256, smem, st>>>(y, y_bs, y_ld, z, z_bs, z_ld, w, bias, T, C, scale, K, dilation, pad, tile);
-  } else {
-    cudaFuncSetAttribute(spk_res2net_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    spk_res2net_kernel<1><<<grid, 256, smem, st>>>(y, y_bs, y_ld, z, z_bs, z_ld, w, bias, T, C, scale, K, dilation, pad, tile);
-  }
+  const auto kern = C % 4 == 0 ? spk_res2net_kernel<4> : spk_res2net_kernel<1>;
+  B2A_SMEM_OPTIN(kern, smem);
+  kern<<<grid, 256, smem, st>>>(y, y_bs, y_ld, z, z_bs, z_ld, w, bias, T, C, scale, K, dilation, pad, tile);
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }

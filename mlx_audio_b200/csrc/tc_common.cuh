@@ -7,6 +7,11 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+// TMA descriptor of a 16-bit (fp16 or bf16) tensor of `rank` (2 or 3) dims, box 128B-swizzled (api.cu).  dims and box innermost first,
+// byte strides of dims 1 .. rank-1; reads past the end return zeros.  0, the CUresult of the encode, or -1 when the driver has no
+// cuTensorMapEncodeTiled.
+int b2a_tmap16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, bool f16);
+
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -154,8 +154,7 @@ extern "C" int32_t b2a_vocos_dwnorm(const float* x, int64_t x_bs, int64_t x_ld, 
   __nv_bfloat16 *eh = (__nv_bfloat16*)hi, *el = (__nv_bfloat16*)lo;
 #define DN_LAUNCH(NV, ADA)                                                                                                      \
   do {                                                                                                                          \
-    static bool attr = false;                                                                                                   \
-    if (!attr) { cudaFuncSetAttribute(vocos_dwnorm_kernel<NV, ADA>, cudaFuncAttributeMaxDynamicSharedMemorySize, 30 * 1024 * 4); attr = true; } \
+    B2A_SMEM_OPTIN((vocos_dwnorm_kernel<NV, ADA>), 30 * 1024 * 4);                                                              \
     vocos_dwnorm_kernel<NV, ADA><<<grid, DN_THREADS, smem, st>>>(x, x_bs, x_ld, L, C, dw_w, dw_b, K, w, b, ada, ada_bs, eps, y, y_bs, y_ld, eh, el); \
   } while (0)
   if (C <= 512) { if (ada) DN_LAUNCH(4, true); else DN_LAUNCH(4, false); }
@@ -176,12 +175,7 @@ extern "C" int32_t b2a_vocos_istft_head(const float* h, int64_t h_bs, int64_t h_
   B2A_CHECK_ARG(out_bs >= nout, "output rows shorter than (T - 1) * hop");
   if (nout == 0) return B2A_OK;
   const size_t smem = (size_t)(n_fft + (n_fft >> 4) + HD_FCH * (n_fft / 2 + 1)) * sizeof(float2);
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(vocos_istft_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)((2048 + 128 + HD_FCH * 1025) * sizeof(float2)));
-    attr = true;
-  }
+  B2A_SMEM_OPTIN(vocos_istft_head_kernel, (2048 + 128 + HD_FCH * 1025) * sizeof(float2));
   const dim3 grid(cdiv(nout, HD_RUN), B);
   vocos_istft_head_kernel<<<grid, HD_RUN, smem, (cudaStream_t)stream>>>(h, h_bs, h_ld, T, n_fft, hop, window, out, out_bs, nout);
   B2A_CHECK_LAUNCH();
@@ -194,8 +188,7 @@ extern "C" int32_t b2a_vocos_logmel(const float* x, int64_t x_bs, int32_t B, int
   B2A_CHECK_ARG(n > VOCOS_MEL_PAD, "reflect padding needs more than 512 samples");
   B2A_CHECK_ARG(frames == n / MEL_HOP, "frames must be n // 256 (the stft's last frame is dropped)");
   const size_t smem = spk_logmel_smem_bytes();
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(spk_logmel_kernel<VOCOS_MEL_PAD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+  B2A_SMEM_OPTIN((spk_logmel_kernel<VOCOS_MEL_PAD, false>), smem);
   dim3 grid(cdiv(frames, MEL_FT), B);
   spk_logmel_kernel<VOCOS_MEL_PAD, false><<<grid, 256, smem, (cudaStream_t)stream>>>(x, x_bs, n, window, filters, n_mels, frames, out);
   B2A_CHECK_LAUNCH();

@@ -615,7 +615,7 @@ def test_split_k_workspace_fallback_and_rearm(small_ws):
 
 
 # --------------------------------------------------------------------------------------------------------------- per-process switches
-# B2A_FUSED_PDL is read once per process, so it runs in a child process that writes its results to a file.
+# B2A_PDL is read once per process, so it runs in a child process that writes its results to a file.
 _PDL_CHAIN = Case("pdl_chain", 1, 300, 256, 256, 3)
 
 
@@ -648,9 +648,9 @@ def _run_child(env, tmp_path):
 
 
 def test_pdl_switch_off_identical(ops, tmp_path):
-    """B2A_FUSED_PDL=0: a dependent chain launched without programmatic dependent launch gives the same bits."""
+    """B2A_PDL=0: a dependent chain launched without programmatic dependent launch gives the same bits."""
     default = _pdl_chain()
-    child = _run_child({"B2A_FUSED_PDL": "0"}, tmp_path)
+    child = _run_child({"B2A_PDL": "0"}, tmp_path)
     assert default["ksplit"][0] > 1 and np.isfinite(default["y"]).all()
     assert np.array_equal(child["y"], default["y"])
 
