@@ -398,16 +398,18 @@ __global__ void randn_advance_kernel(uint64_t* state, uint64_t by) { state[1] +=
 }  // namespace
 
 extern "C" int32_t b2a_randn(float* out, int64_t n, uint64_t seed, uint64_t offset, void* stream) {
-  B2A_CHECK_ARG(out && n >= 0, "bad pointer/size");
-  if (n == 0) return B2A_OK;
+  B2A_CHECK_ARG(n >= 0, "bad pointer/size");
+  if (n == 0) return B2A_OK;                 // before the pointer check: an empty CUDA tensor has a null data pointer
+  B2A_CHECK_ARG(out, "bad pointer/size");
   randn_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(out, n, seed, offset, nullptr);
   B2A_CHECK_LAUNCH();
   return B2A_OK;
 }
 
 extern "C" int32_t b2a_randn_dev(float* out, int64_t n, uint64_t* state, void* stream) {
-  B2A_CHECK_ARG(out && state && n >= 0, "bad pointer/size");
+  B2A_CHECK_ARG(state && n >= 0, "bad pointer/size");
   if (n == 0) return B2A_OK;
+  B2A_CHECK_ARG(out, "bad pointer/size");
   randn_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(out, n, 0, 0, state);
   randn_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state, (uint64_t)((n + 3) / 4));
   B2A_CHECK_LAUNCH();
