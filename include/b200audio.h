@@ -507,13 +507,15 @@ int32_t b2a_stream_rows(const b2a_rowop_t* ops, int32_t n, void* stream);
  * virtual rows [Lout*stride, H + L), into the other slot of hist: float [2][B][keff-1][Cin] with batch stride hist_bs (>= (keff-1)*Cin),
  * slot (*step_dev & 1) being read -- so the caller flips the parity once per step (b2a_stream_advance) and never concatenates.
  * fresh != 0: the first call of a stream, the history rows are the causal left padding instead -- zeros (pad_mode 0) or the first new
- * row (pad_mode 1, replicate); a fresh call with L == 0 writes nothing. */
+ * row (pad_mode 1, replicate); a fresh call with L == 0 writes nothing.  The padding is a row of the activated input, so a prologue with
+ * act(0) != 0 (sigmoid) needs pad_mode 1; stride <= keff (B2A_E_INVALID otherwise). */
 int32_t b2a_conv1d_stream(const b2a_conv1d_t* p, float* hist, int64_t hist_bs, int32_t H, const int32_t* step_dev, int32_t fresh,
                           void* stream);
 /* b2a_convtr1d_stream: StreamableConvTranspose1d.step (conv.py:315-331) -- y [B, L*stride, Cout] = bias + the transposed conv of the L new
  * rows (scatter rule of b2a_convtr1d_cl, no crop) + tail on the first K - stride rows; tail [B, K - stride, Cout] (batch stride tail_bs,
  * row stride Cout, zero at the start of a stream) is then replaced by output rows [L*stride, L*stride + K - stride) WITHOUT the bias (the
- * reference subtracts it).  Dense or depthwise (groups == Cin == Cout); prologue activation, bias and out_scale only; K - stride <= L*stride. */
+ * reference subtracts it).  Dense or depthwise (groups == Cin == Cout); prologue activation, bias and out_scale only; K - stride <= L*stride.
+ * With K == stride there is no tail and tail may be NULL. */
 int32_t b2a_convtr1d_stream(const b2a_conv1d_t* p, float* tail, int64_t tail_bs, void* stream);
 /* Windowed attention over a ring KV cache (transformer.py:79-112 with the growing KVCache and the context mask), position counter on the
  * device so that a captured step replays without host scalars:

@@ -287,7 +287,10 @@ extern "C" int32_t b2a_conv1d_stream(const b2a_conv1d_t* p, float* hist, int64_t
   B2A_CHECK_ARG(p->pad_mode == 0 || p->pad_mode == 1, "pad_mode must be 0 (zeros) or 1 (edge)");
   B2A_CHECK_ARG(conv_extras_ok(p), "unsupported prologue / epilogue field (pre_scale/shift, snake, emit, accumulate)");
   B2A_CHECK_ARG(!p->res || p->res_div >= 1, "res_div must be >= 1");
+  // Padded rows are zeros of the activated input: a prologue with act(0) != 0 would turn them into act(0) (the carry stores raw rows).
+  B2A_CHECK_ARG(p->pad_mode == 1 || p->pre_act != B2A_ACT_SIGMOID, "a sigmoid prologue needs pad_mode 1 (act(0) != 0)");
   const int keff = (p->K - 1) * p->dilation + 1, V = H + p->L;
+  B2A_CHECK_ARG(p->stride <= keff, "stride longer than the window (keff): the carry would go negative");
   const int lout = V >= keff ? (V - keff) / p->stride + 1 : 0;
   B2A_CHECK_ARG(p->Lout == lout, "Lout must be the number of complete windows of [history | new rows]");
   B2A_CHECK_ARG(V - lout * p->stride <= keff - 1, "history slot too small");
@@ -308,7 +311,7 @@ extern "C" int32_t b2a_conv1d_stream(const b2a_conv1d_t* p, float* hist, int64_t
 }
 
 extern "C" int32_t b2a_convtr1d_stream(const b2a_conv1d_t* p, float* tail, int64_t tail_bs, void* stream) {
-  B2A_CHECK_ARG(p && p->x && p->w && p->y && tail, "null pointer");
+  B2A_CHECK_ARG(p && p->x && p->w && p->y && (tail || p->K == p->stride), "null pointer");     // K == stride: no tail, never touched
   B2A_CHECK_ARG(p->B > 0 && p->L > 0 && p->Cin > 0 && p->Cout > 0 && p->stride > 0 && p->K >= p->stride, "bad shape");
   B2A_CHECK_ARG(p->Lout == p->L * p->stride, "Lout must be L * stride");
   B2A_CHECK_ARG(p->K - p->stride <= p->Lout, "tail longer than the output");

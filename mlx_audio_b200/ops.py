@@ -658,19 +658,36 @@ def _stream_conv_params(x, cw: ConvW, B: int, L: int, lout: int, out, stride: in
 
 
 def conv1d_stream(x: Optional[torch.Tensor], cw: ConvW, hist: torch.Tensor, H: int, step: torch.Tensor, *, B=None, stride=1, dilation=1,
-                  pad_mode=0, fresh=False, pre: Optional[Pre] = None, post_act=0, res=None, res_div=1, out=None) -> torch.Tensor:
+                  pad_mode=0, fresh=False, pre: Optional[Pre] = None, post_act=0, cscale=None, res=None, res_div=1, out=None) -> torch.Tensor:
     """b2a_conv1d_stream: the causal conv of [history (H rows) | x] -> its complete windows [B, Lout, Cout] (possibly 0 rows), the unconsumed
     rows carried into the other slot of ``hist`` float32 [2, B, keff - 1, Cin] (slot ``step[0] & 1`` is read).  ``x`` None = no new rows.
-    Returns the output; the caller's new history length is H + L - Lout * stride."""
+    ``cscale`` float32 [B, Cout] scales the output after post_act.  Returns the output; the caller's new history length is
+    H + L - Lout * stride."""
     L = 0 if x is None else x.shape[1]
     B = x.shape[0] if x is not None else B
     keff = (cw.K - 1) * dilation + 1
     lout = (H + L - keff) // stride + 1 if H + L >= keff else 0
-    if hist.dtype != torch.float32 or not hist.is_contiguous() or hist.shape != (2, B, max(keff - 1, 1), cw.cin):
+    if hist.dtype != torch.float32 or not hist.is_cuda or not hist.is_contiguous() or hist.shape != (2, B, max(keff - 1, 1), cw.cin):
         raise ValueError(f"conv1d_stream: history buffer must be float32 [2, {B}, {max(keff - 1, 1)}, {cw.cin}], got {tuple(hist.shape)}")
+    if step.dtype != torch.int32 or not step.is_cuda or step.numel() < 1:
+        raise ValueError(f"conv1d_stream: step must be an int32 CUDA tensor, got {step.dtype} {step.device}")
+    if L and x.shape[2] != cw.cin:
+        raise ValueError(f"conv1d_stream: input has {x.shape[2]} channels, weight expects {cw.cin}")
+    if res is not None:
+        _chk3(res, "conv1d_stream res")
+        if res.shape[0] != B or res.shape[1] < -(-lout // max(res_div, 1)) or res.shape[2] != cw.cout:
+            raise ValueError(f"conv1d_stream: res must be [{B}, >= ceil({lout} / {res_div}), {cw.cout}], got {tuple(res.shape)}")
     if out is None:
         out = torch.empty(B, lout, cw.cout, device=hist.device, dtype=torch.float32)
+    else:
+        _chk3(out, "conv1d_stream out")
+        if out.shape != (B, lout, cw.cout):
+            raise ValueError(f"conv1d_stream: out has shape {tuple(out.shape)}, expected {(B, lout, cw.cout)}")
     p = _stream_conv_params(x, cw, B, L, lout, out, stride, dilation, pad_mode, pre, post_act, res, res_div)
+    if cscale is not None:
+        if cscale.dtype != torch.float32 or not cscale.is_cuda or cscale.shape != (B, cw.cout) or cscale.stride(1) != 1:
+            raise ValueError(f"conv1d_stream: cscale must be CUDA float32 [{B}, {cw.cout}], got {tuple(cscale.shape)} {cscale.dtype}")
+        p.post_cscale, p.post_cscale_bs = cscale.data_ptr(), cscale.stride(0)
     _call("conv", _lib.lib().b2a_conv1d_stream, 1, C.byref(p), hist.data_ptr(), hist.stride(1), H, step.data_ptr(), int(fresh), _stream())
     return out
 
@@ -680,20 +697,38 @@ def convtr1d_stream(x: torch.Tensor, cw: ConvW, tail: torch.Tensor, *, stride: i
     first rows; ``tail`` then holds the next K - stride rows without the bias."""
     _chk3(x, "convtr1d_stream x")
     B, L, _ = x.shape
-    if not tail.is_contiguous() or tail.shape != (B, cw.K - stride, cw.cout):
-        raise ValueError(f"convtr1d_stream: tail must be contiguous [{B}, {cw.K - stride}, {cw.cout}], got {tuple(tail.shape)}")
+    if tail.dtype != torch.float32 or not tail.is_cuda or not tail.is_contiguous() or tail.shape != (B, cw.K - stride, cw.cout):
+        raise ValueError(f"convtr1d_stream: tail must be contiguous float32 [{B}, {cw.K - stride}, {cw.cout}], got {tuple(tail.shape)}")
     if out is None:
         out = torch.empty(B, L * stride, cw.cout, device=x.device, dtype=torch.float32)
+    else:
+        _chk3(out, "convtr1d_stream out")
+        if out.shape != (B, L * stride, cw.cout):
+            raise ValueError(f"convtr1d_stream: out has shape {tuple(out.shape)}, expected {(B, L * stride, cw.cout)}")
     p = _stream_conv_params(x, cw, B, L, L * stride, out, stride, 1, 0, pre, 0, None, 1)
     _call("conv", _lib.lib().b2a_convtr1d_stream, 1, C.byref(p), tail.data_ptr(), tail.stride(0), _stream())
     return out
+
+
+def _chk_rings(name: str, B: int, hd: int, k_ring: torch.Tensor, v_ring: torch.Tensor, pos: torch.Tensor) -> None:
+    """The ring kernels read rows of exactly H*D floats at one batch stride and capacity, taken from k_ring, for both rings."""
+    for r in (k_ring, v_ring):
+        if r.dtype != torch.float32 or not r.is_cuda or r.dim() != 3 or not r.is_contiguous():
+            raise ValueError(f"{name}: rings must be contiguous CUDA float32 [B, cap, H D] tensors, got {tuple(r.shape)} {r.dtype} {r.device}")
+    if k_ring.shape != v_ring.shape or k_ring.shape[0] != B or k_ring.shape[2] != hd:
+        raise ValueError(f"{name}: rings must both be [{B}, cap, {hd}], got {tuple(k_ring.shape)} and {tuple(v_ring.shape)}")
+    if pos.dtype != torch.int32 or not pos.is_cuda or pos.numel() < 1:
+        raise ValueError(f"{name}: pos must be an int32 CUDA tensor, got {pos.dtype} {pos.device}")
 
 
 def ring_rope_kv(qkv: torch.Tensor, n_heads: int, k_ring: torch.Tensor, v_ring: torch.Tensor, pos: torch.Tensor, *, base: float) -> None:
     """b2a_ring_rope_kv: RoPE (interleaved pairs) of q in place and of k at positions pos[0] + t; k, v into ring rows (pos[0] + t) % cap."""
     _chk3(qkv, "ring_rope_kv qkv")
     B, T, w = qkv.shape
+    if w % (3 * n_heads):
+        raise ValueError(f"ring_rope_kv: qkv width {w} is not 3 x {n_heads} heads")
     D = w // (3 * n_heads)
+    _chk_rings("ring_rope_kv", B, n_heads * D, k_ring, v_ring, pos)
     _call("rope", _lib.lib().b2a_ring_rope_kv, 1, qkv.data_ptr(), qkv.stride(0), qkv.stride(1), B, T, n_heads, D, base, k_ring.data_ptr(),
           v_ring.data_ptr(), k_ring.stride(0), k_ring.shape[1], pos.data_ptr(), _stream())
 
@@ -703,8 +738,15 @@ def ring_attn(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, pos: 
     """b2a_ring_attn: q [B, T, H D] (row-strided view) at positions pos[0] + t against the ring caches [B, cap, H D] -> [B, T, H D]."""
     _chk3(q, "ring_attn q")
     B, T, hd = q.shape
+    if hd % n_heads:
+        raise ValueError(f"ring_attn: q width {hd} is not a multiple of {n_heads} heads")
+    _chk_rings("ring_attn", B, hd, k_ring, v_ring, pos)
     if out is None:
         out = torch.empty(B, T, hd, device=q.device, dtype=torch.float32)
+    else:
+        _chk3(out, "ring_attn out")
+        if out.shape != (B, T, hd):
+            raise ValueError(f"ring_attn: out has shape {tuple(out.shape)}, expected {(B, T, hd)}")
     _call("attention", _lib.lib().b2a_ring_attn, 1, q.data_ptr(), q.stride(0), q.stride(1), k_ring.data_ptr(), v_ring.data_ptr(), k_ring.stride(0),
           k_ring.shape[1], out.data_ptr(), out.stride(0), out.stride(1), B, T, n_heads, hd // n_heads, scale, window, pos.data_ptr(), _stream())
     return out

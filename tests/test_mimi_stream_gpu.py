@@ -1,16 +1,12 @@
-"""Mimi's incremental decode_step / encode_step on the GPU (mimi_stream.cu) at the released size with synthetic weights: each new kernel
-against float64, the streams against the float64 oracle's one-shot slices (oracle/mimi_stream.py, pinned to the reference's own step
-functions) and against the product's one-shot decode / encode."""
-import math
-
+"""Mimi's incremental decode_step / encode_step on the GPU (mimi_stream.cu) at the released size with synthetic weights: the streams
+against the float64 oracle's one-shot slices (oracle/mimi_stream.py, pinned to the reference's own step functions) and against the
+product's one-shot decode / encode.  The kernels themselves are tested in test_stream_kernels_matrix_gpu.py."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
 from mlx_audio_b200 import ops, synth
-from mlx_audio_b200.ops import ACT, Pre
 from oracle import codec as OC
 from oracle import mimi_stream as MS
 
@@ -22,115 +18,11 @@ def rel_rms(a, b):
     return float(torch.sqrt(((a - b) ** 2).mean()) / torch.sqrt((b ** 2).mean()))
 
 
-def _bf(t):
-    return t.to(torch.bfloat16).float()
-
-
 @pytest.fixture(scope="module")
 def mimi():
     from mlx_audio_b200.codec import Mimi, mimi_202407
     P = synth.mimi_weights(OC.MIMI_202407, encoder=True)
     return Mimi(mimi_202407(32), device=DEV).load_weights(P), {k: v.double() for k, v in P.items()}
-
-
-# ------------------------------------------------------------------------------------------------------------------------- kernels
-@pytest.mark.parametrize("K,stride,dil,pad_mode,with_res", [(7, 1, 1, 0, False), (3, 1, 2, 0, True), (8, 4, 1, 0, False), (4, 2, 1, 1, False)])
-def test_conv_stream_equals_the_one_shot_causal_conv(K, stride, dil, pad_mode, with_res):
-    g = torch.Generator().manual_seed(K * 10 + stride)
-    B, Cin, Cout = 2, 48, 40
-    w = _bf(torch.randn(Cout, K, Cin, generator=g) / math.sqrt(K * Cin))
-    bias = torch.randn(Cout, generator=g) * 0.1
-    cw = ops.pack_conv(w, bias, 1, DEV)
-    chunks = [5, 0, 1, 13, 2, 40, 3, 0, 17]
-    n = sum(chunks)
-    x = torch.randn(B, n, Cin, generator=g)
-    keff = (K - 1) * dil + 1
-    pad = keff - stride
-    xp = torch.cat([x[:, :1].expand(B, pad, Cin) if pad_mode else torch.zeros(B, pad, Cin), x], 1).double()
-    ref = F.conv1d(F.elu(xp).transpose(1, 2), w.double().permute(0, 2, 1), bias.double(), stride=stride, dilation=dil).transpose(1, 2)
-    res = torch.randn(B, ref.shape[1], Cout, generator=g) if with_res else None
-    if with_res:
-        ref = ref + res.double()
-    hist = torch.zeros(2, B, keff - 1, Cin, device=DEV)
-    ctr = torch.zeros(2, device=DEV, dtype=torch.int32)
-    H, fresh, a, outs = pad, True, 0, []
-    for c in chunks:
-        xc = x[:, a:a + c].to(DEV) if c else None
-        lo = sum(o.shape[1] for o in outs)
-        lout = (H + c - keff) // stride + 1 if H + c >= keff else 0
-        r = res[:, lo:lo + lout].to(DEV).contiguous() if with_res else None
-        y = ops.conv1d_stream(xc, cw, hist, H, ctr[1:], B=B, stride=stride, dilation=dil, pad_mode=pad_mode, fresh=fresh, pre=Pre(act=ACT["elu"]),
-                              res=r)
-        assert y.shape[1] == lout
-        if not (fresh and c == 0):
-            H += c - lout * stride
-            fresh = False
-        ops.stream_advance(ctr, 0)
-        outs.append(y.cpu())
-        a += c
-    got = torch.cat(outs, 1)
-    assert got.shape == ref.shape
-    assert float((got.double() - ref).abs().max() / ref.abs().max()) < 1e-5
-
-
-@pytest.mark.parametrize("Cin,Cout,K,stride,groups", [(40, 24, 8, 4, 1), (64, 64, 4, 2, 64), (96, 48, 10, 5, 1)])
-def test_convtr_stream_equals_the_one_shot_transposed_conv(Cin, Cout, K, stride, groups):
-    g = torch.Generator().manual_seed(K + Cin)
-    B = 2
-    w = _bf(torch.randn(Cout, K, Cin // groups, generator=g) / math.sqrt(K * Cin / groups))
-    bias = torch.randn(Cout, generator=g) * 0.1
-    cw = ops.pack_conv(w, bias, groups, DEV)
-    chunks = [1, 3, 7, 1, 25, 2]
-    x = torch.randn(B, sum(chunks), Cin, generator=g)
-    pre = Pre(act=ACT["elu"]) if groups == 1 else None
-    xin = F.elu(x.double()) if pre else x.double()
-    wt = w.double().permute(2, 0, 1) if groups == 1 else w.double().permute(0, 2, 1)     # torch: [Cin, Cout/g, K]
-    ref = F.conv_transpose1d(xin.transpose(1, 2), wt, bias.double(), stride=stride, groups=groups).transpose(1, 2)[:, :sum(chunks) * stride]
-    tail = torch.zeros(B, K - stride, Cout, device=DEV)
-    a, outs = 0, []
-    for c in chunks:
-        outs.append(ops.convtr1d_stream(x[:, a:a + c].to(DEV).contiguous(), cw, tail, stride=stride, pre=pre).cpu())
-        a += c
-    got = torch.cat(outs, 1)
-    assert float((got.double() - ref).abs().max() / ref.abs().max()) < 1e-5
-
-
-def _rope64(x, pos, base=10000.0):
-    """Interleaved-pair RoPE in float64 on [T, B, H, D] at positions pos [T]."""
-    D = x.shape[-1]
-    inv = torch.exp(-torch.arange(D // 2, dtype=torch.float64) * (math.log(base) / (D // 2)))
-    ang = pos.double()[:, None, None, None] * inv
-    a, b = x[..., 0::2], x[..., 1::2]
-    out = torch.empty_like(x)
-    out[..., 0::2], out[..., 1::2] = a * ang.cos() - b * ang.sin(), a * ang.sin() + b * ang.cos()
-    return out
-
-
-def test_ring_attention_across_wraps_and_chunks_against_float64():
-    g = torch.Generator().manual_seed(7)
-    B, H, D, win = 2, 8, 64, 250
-    cap = win + 2 * 128 + 2
-    chunks = [1, 3, 50, 2, 256, 100, 1, 1, 200, 7]                     # 621 positions: the ring wraps
-    n = sum(chunks)
-    qkv_all = torch.randn(B, n, 3 * H * D, generator=g)
-    kr, vr = torch.zeros(B, cap, H * D, device=DEV), torch.zeros(B, cap, H * D, device=DEV)
-    ctr = torch.zeros(2, device=DEV, dtype=torch.int32)
-    pos = torch.arange(n)
-    q64 = _rope64(qkv_all[:, :, :H * D].double().reshape(B, n, H, D).transpose(0, 1), pos).transpose(0, 1)
-    k64 = _rope64(qkv_all[:, :, H * D:2 * H * D].double().reshape(B, n, H, D).transpose(0, 1), pos).transpose(0, 1)
-    v64 = qkv_all[:, :, 2 * H * D:].double().reshape(B, n, H, D)
-    i, j = pos[:, None], pos[None, :]
-    mask = torch.where((j <= i) & (i - j < win), 0.0, float("-inf")).double()
-    s = torch.einsum("bihd,bjhd->bhij", q64, k64) * D ** -0.5 + mask
-    ref = torch.einsum("bhij,bjhd->bihd", s.softmax(-1), v64).reshape(B, n, H * D)
-    a = 0
-    for c in chunks:
-        qkv = qkv_all[:, a:a + c].to(DEV).contiguous()
-        ops.ring_rope_kv(qkv, H, kr, vr, ctr, base=10000.0)
-        out = ops.ring_attn(qkv[:, :, :H * D], kr, vr, ctr, n_heads=H, scale=D ** -0.5, window=win)
-        ops.stream_advance(ctr, c)
-        assert rel_rms(out, ref[:, a:a + c]) < 1e-5, (a, c)
-        a += c
 
 
 # ------------------------------------------------------------------------------------------------------------------------- decode
