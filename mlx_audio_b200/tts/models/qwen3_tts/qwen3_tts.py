@@ -6,6 +6,8 @@ loop (:1323-1404) with ``_sample_token`` (:805-860), and ``_decode_chunk`` (:101
 voice cloning from reference audio + its transcript (``_generate_icl`` :2200-2510): the speech-tokenizer encoder turns the reference into
 codes, one prompt row per reference frame (``_prepare_icl_generation_inputs`` :606-803), the same frame loop, and a joint decode of
 [reference | generated] codes with the reference's share cut off (``_decode_icl_generated_codes`` :1085-1112).
+``batch_generate`` (:1577-2060) routes a batch of texts to the continuous-batching session, to the static batch loop with one shared ICL
+reference (per-row frame caps, joint decodes as one decoder batch), or to the batch stream (a chunk per row every interval).
 
 One frame = talker step + first-codebook sample + 15 code-predictor sub-steps (each with its sampler) + next-input
 embedding sum: ~700 small launches.  They are captured ONCE into a CUDA graph; every scalar that changes between frames
@@ -15,6 +17,7 @@ graph and reads back 16 integers per frame for the EOS test (the reference also 
 from __future__ import annotations
 
 import time
+from pathlib import Path
 from typing import Dict, List, Optional
 
 import torch
@@ -363,26 +366,34 @@ class Model:
     def _frame_iter(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, max_tokens: int = 4096, temperature: float = 0.9,
                     top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, u=None, seed: int = 0,
                     use_graph: bool = True, stop_on_eos: bool = True, left_padding=None, batch_mode: bool = False,
-                    trailing_rule: str = "clamp_pad"):
+                    trailing_rule: str = "clamp_pad", caps=None, emit_every: Optional[int] = None):
         """The loop of ``generate_codes`` as a generator: outside batch mode it yields (out, n) after every recorded frame -- ``out``
-        [B, max_tokens, 16] is the device buffer whose first n frames are final -- and returns what ``generate_codes`` returns."""
+        [B, max_tokens, 16] is the device buffer whose first n frames are final -- and returns what ``generate_codes`` returns.
+
+        Batch mode: ``caps`` [B] are per-row frame caps (the ICL rule of qwen3_tts.py:1818-1823, 1925-1932: a row that has recorded its
+        cap is finished, and forced to EOS from the next frame on); rows without caps get ``max_tokens``.  With ``emit_every`` = k the
+        loop yields (out, n, lengths [B] on the host) after every k-th frame -- rows advance in lockstep, so a row can only complete a
+        stream chunk there -- unless every row has finished, in which case the reference breaks before emitting (:1913-1932)."""
         t, cfg, dev = self.talker, self.config.talker_config, self.device
         x = input_embeds.to(dev).float().contiguous()
         B, P, H = x.shape
         g, V = cfg.num_code_groups, cfg.vocab_size
         eos = cfg.codec_eos_token_id
+        batch_mode = batch_mode or left_padding is not None
+        capped = caps is not None
+        caps = [min(int(c), max_tokens) for c in caps] if capped else [max_tokens] * B
+        n_steps = max(caps) if batch_mode else max_tokens          # every row has finished by then: the cache needs no more rows
         if u is None:
             u = torch.rand(max_tokens, g, B, device=dev, generator=self._uniform_stream(seed))
         u = u.to(dev).float().contiguous()
         sp = {"temperature": float(temperature), "top_k": int(top_k), "top_p": float(top_p), "repetition_penalty": float(repetition_penalty),
               "eos": int(eos)}
-        batch_mode = batch_mode or left_padding is not None
         self._kv_start = None
         if left_padding is not None and any(int(v) for v in left_padding):
             self._kv_start = torch.tensor([int(v) for v in left_padding], dtype=torch.int32, device=dev)
         self._finished = torch.zeros(B, dtype=torch.uint8, device=dev) if batch_mode else None
         self._tidx = torch.zeros(B, dtype=torch.int32, device=dev) if batch_mode else None
-        t.reset_cache(B, P + max_tokens + 1)
+        t.reset_cache(B, P + n_steps + 1)
         self._prefill_len = P
         self._trailing = trailing_text_hidden.to(dev).float().expand(B, -1, -1).contiguous() if trailing_text_hidden.shape[0] != B \
             else trailing_text_hidden.to(dev).float().contiguous()
@@ -402,10 +413,12 @@ class Model:
         self._err = torch.zeros(1, dtype=torch.int32, device=dev)
         out = torch.zeros(B, max_tokens, g, dtype=torch.int64, device=dev)
         lengths_dev = torch.zeros(B, dtype=torch.int64, device=dev)
-        done = torch.zeros(B, dtype=torch.bool)
+        caps_dev = torch.tensor(caps, dtype=torch.int64, device=dev)
+        cap_hit = torch.zeros(B, dtype=torch.bool, device=dev)
+        done =torch.zeros(B, dtype=torch.bool)
         n = 0
         graph = None
-        for step in range(max_tokens):
+        for step in range(n_steps):
             self._u.copy_(u[step])
             if step == 0:
                 self._frame(x, sp)                                                   # prefill frame (S = P rows), eager
@@ -442,8 +455,15 @@ class Model:
                 fin = self._finished.bool()
                 out[:, n] = torch.where(fin[:, None], out[:, n], self._codes)
                 lengths_dev += (~fin).to(torch.int64)
+                self._finished.bitwise_or_(torch.ge(lengths_dev, caps_dev, out=cap_hit))
                 n += 1
-                if (step & 7) == 7 and bool(fin.all()):
+                if emit_every and n % emit_every == 0:
+                    state = torch.cat([lengths_dev, self._finished.to(torch.int64)]).cpu()      # the one read per chunk boundary
+                    # without caps a row is never finished by max_tokens in the reference: the last frame still emits
+                    if bool(state[B:].all()) and (capped or n < n_steps):
+                        break
+                    yield out, n, state[:B]
+                elif (step & 7) == 7 and bool(self._finished.all()):
                     break
                 continue
             if stop_on_eos:
@@ -502,6 +522,10 @@ class Model:
         per = [self.prepare_generation_inputs_from_ids(ids, language_id, None if speaker_ids is None else speaker_ids[i],
                                                        instruct_ids=None if instruct_ids is None else instruct_ids[i])
                for i, ids in enumerate(ids_list)]
+        return self._pad_batch(per)
+
+    def _pad_batch(self, per):
+        """Per-row (input_embeds [1,P_b,H], trailing [1,n_b,H], tts_pad [1,1,H]) -> the padded batch of ``_prepare_batch_inputs``."""
         pad = per[0][2]
         pmax = max(e.shape[1] for e, _, _ in per)
         tmax = max(tr.shape[1] for _, tr, _ in per)
@@ -517,37 +541,37 @@ class Model:
 
     def batch_generate_from_ids(self, ids_list, *, language_id=None, speaker_ids=None, temperature: float = 0.9, max_tokens: int = 4096,
                                 top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, seed: int = 0, u=None,
-                                stream: bool = False, **kwargs):
+                                stream: bool = False, streaming_interval: float = 2.0, **kwargs):
         """``Model.batch_generate`` (qwen3_tts.py:1651-2060) for already-tokenised texts, one BatchGenerationResult per sequence.
 
         ``stream=False`` (the reference's default) follows its batch session (continuous_batching.py): every row generates exactly what it
         would generate alone from its own uniform stream (standard trailing-text rule), and is decoded by ``_decode_generated_codes`` --
         15-frame chunks with 5 frames of left context (qwen3_tts.py:1050-1083).  ``stream=True`` follows the streaming branch
-        (qwen3_tts.py:1861-2040) with one final chunk per row: finished rows forced to EOS, clamp-pad trailing rule, one decode of the whole
-        row (chunks of 300 + 25 context)."""
+        (qwen3_tts.py:1861-2029): finished rows forced to EOS, clamp-pad trailing rule, and a chunk per row every ``streaming_interval``
+        seconds of frames, then each row's remainder as its final chunk (``_stream_batch``)."""
         from ..base import BatchGenerationResult
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
         x, trailing, pad, left = self.prepare_batch_inputs_from_ids(ids_list, language_id, speaker_ids)
-        codes, lengths = self.generate_codes(x, trailing, pad, max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
-                                             repetition_penalty=repetition_penalty, seed=seed, u=u, left_padding=left, batch_mode=True,
-                                             trailing_rule="clamp_pad" if stream else "standard")
-        seqs = [codes[b, : int(lengths[b])] for b in range(codes.shape[0])]
+        gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed,
+                   u=u, left_padding=left, batch_mode=True)
         if stream:
-            audios, _ = self.speech_tokenizer.batch_decode([s_ for s_ in seqs if s_.shape[0] > 0])
-        else:
-            # rows of equal length share their decode launches: the chunks of _decode_generated_codes do not interact, so chunk j of every
-            # row goes through the vocoder as one batch (identical samples; 8 rows x 3 chunks: 24 decoder passes -> 2)
-            live = [s_ for s_ in seqs if s_.shape[0] > 0]
-            by_len: Dict[int, List[int]] = {}
-            for i, s_ in enumerate(live):
-                by_len.setdefault(int(s_.shape[0]), []).append(i)
-            audios = [None] * len(live)
-            for n_, idxs in by_len.items():
-                wav = self.speech_tokenizer.decoder.chunked_decode(torch.stack([live[i] for i in idxs]).transpose(1, 2), chunk_size=15, left_context_size=5)
-                for j, i in enumerate(idxs):
-                    audios[i] = wav[j, 0]
+            yield from self._stream_batch(x, trailing, pad, gen, streaming_interval, t0)
+            return
+        codes, lengths = self.generate_codes(x, trailing, pad, trailing_rule="standard", **gen)
+        seqs = [codes[b, : int(lengths[b])] for b in range(codes.shape[0])]
+        # rows of equal length share their decode launches: the chunks of _decode_generated_codes do not interact, so chunk j of every
+        # row goes through the vocoder as one batch (identical samples; 8 rows x 3 chunks: 24 decoder passes -> 2)
+        live = [s_ for s_ in seqs if s_.shape[0] > 0]
+        by_len: Dict[int, List[int]] = {}
+        for i, s_ in enumerate(live):
+            by_len.setdefault(int(s_.shape[0]), []).append(i)
+        audios = [None] * len(live)
+        for n_, idxs in by_len.items():
+            wav = self.speech_tokenizer.decoder.chunked_decode(torch.stack([live[i] for i in idxs]).transpose(1, 2), chunk_size=15, left_context_size=5)
+            for j, i in enumerate(idxs):
+                audios[i] = wav[j, 0]
         torch.cuda.synchronize(self.device)
         dt = time.perf_counter() - t0
         it = iter(audios)
@@ -557,8 +581,229 @@ class Model:
             a = next(it)
             yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=int(s_.shape[0]),
                                         audio_duration=format_duration(a.shape[0] / self.sample_rate), processing_time_seconds=dt,
-                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9, is_streaming_chunk=stream,
-                                        is_final_chunk=stream)
+                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+
+    def _stream_batch(self, x, trailing, pad, gen: dict, streaming_interval: float, t0: float):
+        """The streaming branch of the static batch loop (qwen3_tts.py:1943-2029): once a row has ``max(1, int(streaming_interval * 12.5))``
+        undecoded frames it emits them, decoded by ``chunked_decode`` behind up to 25 frames of context whose samples are dropped (the
+        reference hard-codes the 25); after the loop every row with undecoded frames emits them as its final chunk.  The host reads the
+        row lengths only at chunk boundaries (``_frame_iter(emit_every=...)``)."""
+        chunk = max(1, int(streaming_interval * 12.5))
+        B = x.shape[0]
+        decoded = [0] * B
+        frames = self._frame_iter(x, trailing, pad, emit_every=chunk, **gen)
+        while True:
+            try:
+                out, n, lengths = next(frames)
+            except StopIteration as stop:
+                out, lengths = stop.value
+                break
+            yield from self._emit_batch_chunks(out, [b for b in range(B) if int(lengths[b]) == n], decoded, [n] * B, False, t0)
+        ends = [int(v) for v in lengths]
+        yield from self._emit_batch_chunks(out, [b for b in range(B) if ends[b] > decoded[b]], decoded, ends, True, t0)
+
+    def _emit_batch_chunks(self, out, rows, decoded, ends, final: bool, t0: float):
+        """One stream step of ``_stream_batch``: frames [decoded[b], ends[b]) of every row b in ``rows``, in row order.  Rows with equal
+        context and chunk lengths go through one ``chunked_decode`` call (at an in-loop step that is every emitting row)."""
+        from ..base import BatchGenerationResult
+        up = self.speech_tokenizer.decode_upsample_rate
+        groups: Dict[tuple, List[int]] = {}
+        for b in rows:
+            groups.setdefault((min(25, decoded[b]), ends[b] - decoded[b]), []).append(b)
+        audio = {}
+        for (ctx, new), members in groups.items():
+            codes = torch.stack([out[b, decoded[b] - ctx: ends[b]] for b in members])                  # [R, ctx + new, G]
+            wav = self.speech_tokenizer.decoder.chunked_decode(codes.transpose(1, 2))[:, 0]
+            for i, b in enumerate(members):
+                audio[b] = wav[i, ctx * up:] if ctx * up < wav.shape[1] else wav[i]
+        torch.cuda.synchronize(self.device)
+        for b in rows:
+            new = ends[b] - decoded[b]
+            decoded[b] = ends[b]
+            a = audio[b]
+            yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=new,
+                                        audio_duration=format_duration(a.shape[0] / self.sample_rate),
+                                        processing_time_seconds=time.perf_counter() - t0,
+                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9, is_streaming_chunk=True,
+                                        is_final_chunk=final)
+
+    # ------------------------------------------------------------------ batch_generate: requests, routes, ICL
+    @staticmethod
+    def _same_shared_ref_value(left, right) -> bool:
+        """qwen3_tts.py:1577-1580: paths are the same reference when their strings are; arrays only when they are the same object."""
+        if isinstance(left, (str, Path)) and isinstance(right, (str, Path)):
+            return str(left) == str(right)
+        return left is right
+
+    @staticmethod
+    def _normalize_shared_batch_refs(batch_size: int, *, ref_audio=None, ref_text: Optional[str] = None, ref_audios=None, ref_texts=None):
+        """qwen3_tts.py:1582-1649: resolve one shared in-context reference (audio, transcript) for the whole batch from the scalar and the
+        per-text list arguments, with the reference's errors.  Returns (ref_audio, ref_text), both None without a reference."""
+        def shared_from_list(name, values):
+            if values is None:
+                return None
+            if len(values) != batch_size:
+                raise ValueError(f"{name} length ({len(values)}) must match texts length ({batch_size})")
+            present = [v for v in values if v is not None]
+            if not present:
+                return None
+            if len(present) != batch_size:
+                raise ValueError(f"Qwen3-TTS batch_generate requires {name} for every text when using reference cloning")
+            shared = present[0]
+            for v in present[1:]:
+                if not Model._same_shared_ref_value(shared, v):
+                    raise ValueError(f"Qwen3-TTS batch_generate currently supports only one shared {name[:-1]} across the whole batch")
+            return shared
+
+        list_audio = shared_from_list("ref_audios", ref_audios)
+        list_text = shared_from_list("ref_texts", ref_texts)
+        if list_audio is not None:
+            if ref_audio is not None and not Model._same_shared_ref_value(ref_audio, list_audio):
+                raise ValueError("ref_audio and ref_audios must refer to the same shared reference")
+            ref_audio = list_audio
+        if list_text is not None:
+            if ref_text is not None and ref_text != list_text:
+                raise ValueError("ref_text and ref_texts must refer to the same shared reference")
+            ref_text = list_text
+        if ref_audio is None and ref_text is None:
+            return None, None
+        if ref_audio is None or ref_text is None:
+            raise ValueError("Qwen3-TTS batch reference cloning requires both ref_audio and ref_text")
+        if isinstance(ref_audio, (str, Path)):
+            raise NotImplementedError("batch_generate: file decoding (audio_io) is outside the accelerated path; pass 24 kHz samples")
+        return ref_audio, ref_text
+
+    @staticmethod
+    def _batch_request(batch_size: int, voices=None, instructs=None, ref_audio=None, ref_text=None, ref_audios=None, ref_texts=None,
+                       has_encoder: bool = False):
+        """The request checks of batch_generate (qwen3_tts.py:1699-1739): per-text lists of the right length, one shared reference, and
+        no voices / instructs / encoder-less speech tokenizer with it.  Returns (voices, instructs, ref_audio, ref_text, use_icl)."""
+        if voices is None:
+            voices = [None] * batch_size
+        elif len(voices) != batch_size:
+            raise ValueError(f"voices length ({len(voices)}) must match texts length ({batch_size})")
+        if instructs is None:
+            instructs = [None] * batch_size
+        elif len(instructs) != batch_size:
+            raise ValueError(f"instructs length ({len(instructs)}) must match texts length ({batch_size})")
+        ref_audio, ref_text = Model._normalize_shared_batch_refs(batch_size, ref_audio=ref_audio, ref_text=ref_text, ref_audios=ref_audios,
+                                                                 ref_texts=ref_texts)
+        use_icl = ref_audio is not None and ref_text is not None
+        if use_icl:
+            if not has_encoder:
+                raise ValueError("Qwen3-TTS batch reference cloning requires a speech tokenizer encoder")
+            if any(v is not None for v in voices):
+                raise ValueError("Qwen3-TTS batch reference cloning does not support voices")
+            if any(i is not None for i in instructs):
+                raise ValueError("Qwen3-TTS batch reference cloning does not support instructs")
+        return voices, instructs, ref_audio, ref_text, use_icl
+
+    def batch_generate_icl_from_ids(self, target_ids_list, ref_ids, *, ref_audio=None, ref_codes=None, speaker_embed=None, language_id=None,
+                                    row_max_tokens=None, temperature: float = 0.9, max_tokens: int = 4096, top_k: int = 50, top_p: float = 1.0,
+                                    repetition_penalty: float = 1.5, seed: int = 0, u=None, stream: bool = False,
+                                    streaming_interval: float = 2.0, **kwargs):
+        """The in-context branch of ``Model.batch_generate`` (qwen3_tts.py:1798-2060) for already-tokenised texts sharing one reference
+        (ids as in ``prepare_icl_generation_inputs_from_ids``).  The reference is encoded (``ref_codes`` [1, 16, T_ref], unless given) and
+        its x-vector computed once for the call; every row gets its own in-context prompt, the prompts are left-padded into one batch, and
+        row b stops on EOS or after ``row_max_tokens[b]`` frames (default ``max_tokens``).  ``u`` [max_tokens, 16, B] injects the uniforms.
+        Yields one BatchGenerationResult per row with frames: [ref | generated] decoded together (one decoder batch for all rows), trimmed
+        to the valid length, the reference's share cut off; or with ``stream=True`` chunks of the generated codes (``_stream_batch``)."""
+        from ..base import BatchGenerationResult
+        if self.speech_tokenizer is None:
+            raise ValueError("Speech tokenizer not loaded")
+        t0 = time.perf_counter()
+        if ref_codes is None:
+            if ref_audio is None:
+                raise ValueError("batch_generate_icl_from_ids: pass ref_audio or ref_codes")
+            ref_codes = self.encode_reference(ref_audio)
+        if speaker_embed is None and ref_audio is not None and self.speaker_encoder is not None:
+            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        per = [self.prepare_icl_generation_inputs_from_ids(ids, ref_ids, ref_codes, language_id, speaker_embed) for ids in target_ids_list]
+        x, trailing, pad, left = self._pad_batch(per)
+        gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed,
+                   u=u, left_padding=left, batch_mode=True, caps=row_max_tokens if row_max_tokens is not None else [max_tokens] * len(per))
+        if stream:
+            yield from self._stream_batch(x, trailing, pad, gen, streaming_interval, t0)
+            return
+        codes, lengths = self.generate_codes(x, trailing, pad, **gen)
+        dt = time.perf_counter() - t0
+        rows = [b for b in range(codes.shape[0]) if int(lengths[b]) > 0]
+        audios = self._decode_icl_batch([codes[b, : int(lengths[b])] for b in rows], ref_codes)
+        for b, a in zip(rows, audios):
+            yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=int(lengths[b]),
+                                        audio_duration=format_duration(a.shape[0] / self.sample_rate), processing_time_seconds=dt,
+                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+
+    def _icl_reference(self, ref_audio, ref_text):
+        """(ref codes [1, 16, T], transcript ids) of a reference, cached on (ref_text, (size, sum) of ref_audio) (qwen3_tts.py:639-664)."""
+        a = ref_audio if isinstance(ref_audio, torch.Tensor) else torch.as_tensor(ref_audio)
+        key = (ref_text, (int(a.numel()), float(a.sum())))
+        if key not in self._icl_cache:
+            self._icl_cache[key] = (self.encode_reference(a), self.tokenizer.encode(f"<|im_start|>assistant\n{ref_text}<|im_end|>\n"))
+        return a, self._icl_cache[key]
+
+    def _language_id(self, lang_code: str):
+        cfg = self.config.talker_config
+        if lang_code.lower() != "auto" and cfg.codec_language_id and lang_code.lower() in cfg.codec_language_id:
+            return cfg.codec_language_id[lang_code.lower()]
+        return None
+
+    def batch_generate(self, texts: List[str], voices: Optional[List[Optional[str]]] = None, instructs: Optional[List[Optional[str]]] = None,
+                       ref_audio=None, ref_text: Optional[str] = None, ref_audios=None, ref_texts: Optional[List[Optional[str]]] = None,
+                       temperature: float = 0.9, lang_code: str = "auto", max_tokens: int = 4096, top_k: int = 50, top_p: float = 1.0,
+                       repetition_penalty: float = 1.05, stream: bool = False, streaming_interval: float = 2.0, streaming_context_size: int = 25,
+                       verbose: bool = False, seed: Optional[int] = None, **kwargs):
+        """Model.batch_generate (qwen3_tts.py:1651-2060): BatchGenerationResults for several texts generated as one batch.
+        ``stream=False`` without a reference runs the continuous-batching session (:1741-1796); with one shared reference
+        (``ref_audio`` + ``ref_text``, or the per-text aliases ``ref_audios`` / ``ref_texts`` naming the same reference) the in-context
+        static batch (``batch_generate_icl_from_ids``), each row capped at ``min(max_tokens, max(75, 6 * len(encode(text))))`` frames and
+        the repetition penalty raised to at least 1.5; ``stream=True`` the static batch with a chunk per row every ``streaming_interval``
+        seconds.  ``streaming_context_size`` is accepted and, as in the reference, the stream context is 25 frames whatever it says."""
+        if self.speech_tokenizer is None:
+            raise ValueError("Speech tokenizer not loaded")
+        B = len(texts)
+        if B == 0:
+            return
+        voices, instructs, ref_audio, ref_text, use_icl = self._batch_request(B, voices, instructs, ref_audio, ref_text, ref_audios, ref_texts,
+                                                                              self.speech_tokenizer.has_encoder)
+        if self.tokenizer is None:
+            raise ValueError("Tokenizer not loaded. Call post_load_hook first.")
+        gen = dict(temperature=temperature, max_tokens=max_tokens, top_k=top_k, top_p=top_p, seed=seed, stream=stream,
+                   streaming_interval=streaming_interval)
+        if use_icl:
+            a, (ref_codes, ref_ids) = self._icl_reference(ref_audio, ref_text)
+            target = [self.tokenizer.encode(f"<|im_start|>assistant\n{t}<|im_end|>\n<|im_start|>assistant\n") for t in texts]
+            caps = [min(max_tokens, max(75, len(self.tokenizer.encode(t)) * 6)) for t in texts]      # raw text, no template (:1818-1823)
+            yield from self.batch_generate_icl_from_ids(target, ref_ids, ref_audio=a, ref_codes=ref_codes, language_id=self._language_id(lang_code),
+                                                        row_max_tokens=caps, repetition_penalty=max(repetition_penalty, 1.5), **gen)
+            return
+        if stream:
+            per = [self._prepare_generation_inputs(t, language=lang_code, speaker=v, instruct=i) for t, v, i in zip(texts, voices, instructs)]
+            x, trailing, pad, left = self._pad_batch(per)
+            yield from self._stream_batch(x, trailing, pad, dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
+                                                                 repetition_penalty=repetition_penalty, seed=seed, left_padding=left,
+                                                                 batch_mode=True), streaming_interval, time.perf_counter())
+            return
+        from ...continuous import TTSBatchItem, TTSBatchOptions
+        from ..base import BatchGenerationResult
+        session = self.create_tts_batch_session(TTSBatchOptions(temperature=temperature, top_p=top_p, top_k=top_k, repetition_penalty=repetition_penalty,
+                                                                max_tokens=max_tokens, lang_code=lang_code, stream=False,
+                                                                streaming_interval=streaming_interval, max_batch_size=B, verbose=verbose))
+        session.add([TTSBatchItem(sequence_id=i, text=t, voice=voices[i], instruct=instructs[i]) for i, t in enumerate(texts)])
+        t0 = time.perf_counter()
+        while not session.idle:
+            for ev in session.step():
+                if ev.error is not None:
+                    raise ev.error
+                if ev.audio is None or ev.samples <= 0:
+                    continue
+                yield BatchGenerationResult(audio=ev.audio, sequence_idx=ev.sequence_id, samples=ev.samples, sample_rate=ev.sample_rate,
+                                            token_count=ev.token_count,
+                                            audio_duration=ev.metadata.get("audio_duration", format_duration(ev.samples / self.sample_rate)),
+                                            processing_time_seconds=ev.metadata.get("processing_time_seconds", time.perf_counter() - t0),
+                                            peak_memory_usage=ev.metadata.get("peak_memory_usage",
+                                                                              torch.cuda.max_memory_allocated(self.device) / 1e9),
+                                            is_streaming_chunk=ev.is_streaming_chunk, is_final_chunk=ev.is_final_chunk)
 
     # ------------------------------------------------------------------ decode + public generate
     @torch.no_grad()
@@ -691,33 +936,40 @@ class Model:
     def _decode_icl_generated_codes(self, gen_codes: torch.Tensor, ref_codes: torch.Tensor) -> torch.Tensor:
         """qwen3_tts.py:1085-1112: gen_codes [n, 16] -> the target's audio: [ref | generated] decoded together, trimmed to the valid length
         (frames whose first code is > 0), then int(T_ref / total * samples) samples of reference cut off the front."""
+        return self._decode_icl_batch([gen_codes], ref_codes)[0]
+
+    @torch.no_grad()
+    def _decode_icl_batch(self, gen_list, ref_codes) -> List[torch.Tensor]:
+        """``_decode_icl_generated_codes`` for several rows [n_b, 16] of one reference: the rows [ref | gen_b] go through the decoder as one
+        batch, right-padded with code 0.  Chunk boundaries count from frame 0 and the decoder is causal, so padding after a row's end does
+        not reach its frames; the valid lengths and cuts are each row's own."""
+        up = self.speech_tokenizer.decode_upsample_rate
         ref_t = torch.as_tensor(ref_codes, dtype=torch.int64).to(self.device)[0].transpose(0, 1)
-        full = torch.cat([ref_t, gen_codes.to(self.device)], dim=0)[None]
-        wav, lengths = self.speech_tokenizer.decode(full)
-        audio = wav[0]
-        valid = int(lengths[0])
-        if 0 < valid < audio.shape[0]:
-            audio = audio[:valid]
-        cut = int(ref_t.shape[0] / max(full.shape[1], 1) * audio.shape[0])
-        return audio[cut:] if 0 < cut < audio.shape[0] else audio
+        totals = [ref_t.shape[0] + int(c.shape[0]) for c in gen_list]
+        full = torch.zeros(len(gen_list), max(totals), ref_t.shape[1], dtype=torch.int64, device=self.device)
+        full[:, : ref_t.shape[0]] = ref_t
+        for i, c in enumerate(gen_list):
+            full[i, ref_t.shape[0]: totals[i]] = c.to(self.device)
+        wav = self.speech_tokenizer.decoder.chunked_decode(full.transpose(1, 2))[:, 0]
+        valid = ((full[..., 0] > 0).sum(dim=1) * up).tolist()             # padding is code 0: it never counts as valid
+        audios = []
+        for i, total in enumerate(totals):
+            audio = wav[i, : total * up]
+            if 0 < valid[i] < audio.shape[0]:
+                audio = audio[: valid[i]]
+            cut = int(ref_t.shape[0] / max(total, 1) * audio.shape[0])
+            audios.append(audio[cut:] if 0 < cut < audio.shape[0] else audio)
+        return audios
 
     def _generate_icl(self, text, ref_audio, ref_text, language, stream, streaming_interval, **gen):
         """_generate_icl (qwen3_tts.py:2200-2510): the text is one segment; the reference's codes (and transcript ids) are cached on
         (ref_text, (size, sum) of ref_audio), so a repeated reference does not run the encoder again (:639-664)."""
         if self.tokenizer is None:
             raise ValueError("Tokenizer not loaded. Call post_load_hook first.")
-        cfg = self.config.talker_config
-        a = ref_audio if isinstance(ref_audio, torch.Tensor) else torch.as_tensor(ref_audio)
-        key = (ref_text, (int(a.numel()), float(a.sum())))
-        if key not in self._icl_cache:
-            self._icl_cache[key] = (self.encode_reference(a), self.tokenizer.encode(f"<|im_start|>assistant\n{ref_text}<|im_end|>\n"))
-        ref_codes, ref_ids = self._icl_cache[key]
+        a, (ref_codes, ref_ids) = self._icl_reference(ref_audio, ref_text)
         target_ids = self.tokenizer.encode(f"<|im_start|>assistant\n{text}<|im_end|>\n<|im_start|>assistant\n")
-        language_id = None
-        if language.lower() != "auto" and cfg.codec_language_id and language.lower() in cfg.codec_language_id:
-            language_id = cfg.codec_language_id[language.lower()]
-        yield from self.generate_icl_from_ids(target_ids, ref_ids, ref_audio=a, ref_codes=ref_codes, language_id=language_id, stream=stream,
-                                              streaming_interval=streaming_interval, **gen)
+        yield from self.generate_icl_from_ids(target_ids, ref_ids, ref_audio=a, ref_codes=ref_codes, language_id=self._language_id(language),
+                                              stream=stream, streaming_interval=streaming_interval, **gen)
 
     def _generate_segments(self, text, split_pattern, speaker, language, instruct, stream=False, streaming_interval=2.0, ref_audio=None, **gen):
         if self.speech_tokenizer is None:
