@@ -347,7 +347,7 @@ int32_t b2a_sample_token(const float* logits, int64_t logits_bs, int32_t B, int3
                          float* filtered_out, uint8_t* finished, int32_t eos, void* stream);
 
 /* ---- autoregressive LM step (Qwen3-TTS talker / code predictor, tts/models/qwen3_tts/talker.py) -----------------------
- * All position-dependent scalars may come from device memory (base_dev, step_dev) so that one captured CUDA graph replays
+ * All position-dependent scalars may come from device memory (base_dev, tidx) so that one captured CUDA graph replays
  * every frame of Model.generate's loop (qwen3_tts.py:1323-1404) without host round trips.
  *
  * b2a_gemv_bf16: y[m, n] = sum_k W[n,k] xn[m,k] (+ bias[n]) (+ res[m,n]) for M <= 8 activation rows -- nn.Linear at decode
@@ -398,14 +398,14 @@ int32_t b2a_attn_prefill(const float* q, int64_t q_bs, int64_t q_ss, const float
 /* y[r, i] = silu(gate) * up (talker.py:319-321, speech_tokenizer.py:321-322) for the batched (prefill) path: x [rows, 2I] holds
  * (gate | up) halves, or interleaved (gate_0, up_0, gate_1, ...) pairs -- the row order b2a_gemv_bf16 mode 1 uses. */
 int32_t b2a_swiglu(const float* x, int64_t x_ld, int64_t rows, int32_t I, int32_t interleaved, float* y, int64_t y_ld, void* stream);
-/* Next talker input (qwen3_tts.py:1383-1398): out[b] = text(b) + sum_g tables[g][codes[b,g]], text(b) = text[b, step] while
- * step = *step_dev - step_sub < n_text, else pad (tts_pad_embed); text/pad NULL = 0.  tables_dev / bins_dev are DEVICE arrays
- * of G table pointers / table sizes; an out-of-range code sets *err_flag_dev.  tidx != NULL selects the batch rule of
+/* Next talker input (qwen3_tts.py:1383-1398): out[b] = text(b) + sum_g tables[g][codes[b,g]].  tables_dev / bins_dev are DEVICE
+ * arrays of G table pointers / table sizes; an out-of-range code sets *err_flag_dev.  text(b) follows the batch rule of
  * _next_batch_input_embeds(pad_when_index_clamped=True) (qwen3_tts.py:993-1015): text row min(tidx[b], n_text-1), replaced by pad
- * when that is >= n_text-1; afterwards tidx[b] += 1 for rows that are not finished. */
+ * (tts_pad_embed) when that is >= n_text-1; afterwards tidx[b] += 1 for rows that are not finished.  text and tidx are given
+ * together or not at all; without them text(b) = pad (NULL = 0). */
 int32_t b2a_embed_sum(const int64_t* codes, int64_t codes_bs, int32_t B, int32_t G, int32_t dim, const float* const* tables_dev,
                       const int32_t* bins_dev, const float* text, int64_t text_bs, int64_t text_ss, int32_t n_text,
-                      const float* pad, const int32_t* step_dev, int32_t step_sub, float* out, int64_t out_bs,
+                      const float* pad, float* out, int64_t out_bs,
                       int32_t* err_flag_dev, int32_t* tidx, const uint8_t* finished, void* stream);
 /* *p += v on the stream (KVCache.offset bookkeeping, lm/models/cache.py:112-155, kept on the device). */
 int32_t b2a_incr_i32(int32_t* p, int32_t v, void* stream);

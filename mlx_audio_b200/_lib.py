@@ -134,7 +134,7 @@ PROTOTYPES = {
     "b2a_attn_prefill": (i32, [c_f, i64, i64, c_f, c_f, i64, i64, c_f, i64, i64, i32, i32, i32, i32, i32, f32, c_f, i32, c_f, i32, c_f, c_f,
                                C.c_void_p]),
     "b2a_swiglu": (i32, [c_f, i64, i64, i32, i32, c_f, i64, C.c_void_p]),
-    "b2a_embed_sum": (i32, [c_f, i64, i32, i32, i32, c_f, c_f, c_f, i64, i64, i32, c_f, c_f, i32, c_f, i64, c_f, c_f, c_f, C.c_void_p]),
+    "b2a_embed_sum": (i32, [c_f, i64, i32, i32, i32, c_f, c_f, c_f, i64, i64, i32, c_f, c_f, i64, c_f, c_f, c_f, C.c_void_p]),
     "b2a_incr_i32": (i32, [c_f, i32, C.c_void_p]),
     "b2a_slot_advance": (i32, [c_f, c_f, c_f, c_f, c_f, i32, c_f, i64, c_f, i64, c_f, i32, C.c_void_p]),
     "b2a_rvq_decode": (i32, [c_f, i64, i64, i32, i32, i64, c_f, i32, i32, c_f, i64, c_f, C.c_void_p]),

@@ -453,9 +453,9 @@ __global__ void swiglu_kernel(const float* x, int64_t x_ld, int64_t rows, int I,
 struct EmbedSumParams {
   const int64_t* codes; int64_t codes_bs; int B, G, dim;
   const float* const* tables; const int* bins;
-  const float* text; int64_t text_bs, text_ss; int n_text; const float* pad; const int* step_dev; int step_sub;
+  const float* text; int64_t text_bs, text_ss; int n_text; const float* pad;
   float* out; int64_t out_bs; int* err;
-  int* tidx; const uint8_t* finished;              // batch loop: per-row trailing index (advanced for unfinished rows), clamp-pad rule
+  int* tidx; const uint8_t* finished;              // per-row trailing index (advanced for unfinished rows), clamp-pad rule
 };
 __global__ void embed_sum_kernel(const EmbedSumParams p) {
   pdl_launch_dependents();
@@ -471,11 +471,7 @@ __global__ void embed_sum_kernel(const EmbedSumParams p) {
     const int cl = idx < p.n_text - 1 ? idx : p.n_text - 1;
     if (cl >= p.n_text - 1) v = p.pad ? p.pad[d] : 0.f;
     else v = p.text[(int64_t)b * p.text_bs + (int64_t)cl * p.text_ss + d];
-  } else if (p.text || p.pad) {
-    const int step = (p.step_dev ? *p.step_dev : 0) - p.step_sub;
-    if (p.text && step >= 0 && step < p.n_text) v = p.text[(int64_t)b * p.text_bs + (int64_t)step * p.text_ss + d];
-    else if (p.pad) v = p.pad[d];
-  }
+  } else if (p.pad) v = p.pad[d];
   for (int g = 0; g < p.G; g++) {
     const int64_t c = p.codes[(int64_t)b * p.codes_bs + g];
     if (c < 0 || c >= p.bins[g]) { if (p.err) *p.err = 1; continue; }
@@ -587,11 +583,12 @@ extern "C" int32_t b2a_swiglu(const float* x, int64_t x_ld, int64_t rows, int32_
 
 extern "C" int32_t b2a_embed_sum(const int64_t* codes, int64_t codes_bs, int32_t B, int32_t G, int32_t dim,
                                  const float* const* tables_dev, const int32_t* bins_dev, const float* text, int64_t text_bs,
-                                 int64_t text_ss, int32_t n_text, const float* pad, const int32_t* step_dev, int32_t step_sub,
-                                 float* out, int64_t out_bs, int32_t* err_flag_dev, int32_t* tidx, const uint8_t* finished, void* stream) {
+                                 int64_t text_ss, int32_t n_text, const float* pad, float* out, int64_t out_bs,
+                                 int32_t* err_flag_dev, int32_t* tidx, const uint8_t* finished, void* stream) {
   B2A_CHECK_ARG(B > 0 && G >= 0 && dim > 0, "bad shape");
-  B2A_CHECK_ARG(tidx == nullptr || (text != nullptr && n_text > 0), "per-row trailing indices need the trailing text rows");
-  EmbedSumParams p{codes, codes_bs, B, G, dim, tables_dev, bins_dev, text, text_bs, text_ss, n_text, pad, step_dev, step_sub, out, out_bs, err_flag_dev,
+  B2A_CHECK_ARG((tidx == nullptr) == (text == nullptr) && (text == nullptr || n_text > 0),
+                "trailing text rows and per-row trailing indices go together");
+  EmbedSumParams p{codes, codes_bs, B, G, dim, tables_dev, bins_dev, text, text_bs, text_ss, n_text, pad, out, out_bs, err_flag_dev,
                    tidx, finished};
   dim3 grid((dim + 255) / 256, B);
   b2a_launch_pdl(embed_sum_kernel, grid, dim3(256), 0, (cudaStream_t)stream, p);

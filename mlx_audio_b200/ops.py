@@ -1208,9 +1208,13 @@ class EmbedTables:
         self.dim = self.tables[0].shape[1]
 
 
-def embed_sum(codes: torch.Tensor, tabs: EmbedTables, *, text=None, pad=None, step_dev=None, step_sub: int = 0, out=None, err=None,
-              tidx=None, finished=None) -> torch.Tensor:
-    """out[b] = text-or-pad(b) + sum_g tables[g][codes[b,g]]; codes int64 [B,G] (G <= len(tables))."""
+def embed_sum(codes: torch.Tensor, tabs: EmbedTables, *, text=None, pad=None, out=None, err=None, tidx=None,
+              finished=None) -> torch.Tensor:
+    """out[b] = text-or-pad(b) + sum_g tables[g][codes[b,g]]; codes int64 [B,G] (G <= len(tables)).  ``text`` [B, n, H] is read at
+    the per-row trailing indices ``tidx`` int32 [B] (clamp-pad rule; advanced for rows that are not ``finished``); without them
+    every row reads ``pad`` [H] (None = 0)."""
+    if (text is None) != (tidx is None):
+        raise ValueError("embed_sum: text= and tidx= go together")
     assert codes.dtype == torch.int64 and codes.dim() == 2 and codes.stride(1) == 1
     B, G = codes.shape
     assert G <= len(tabs.tables)
@@ -1218,7 +1222,7 @@ def embed_sum(codes: torch.Tensor, tabs: EmbedTables, *, text=None, pad=None, st
         out = torch.empty(B, tabs.dim, device=codes.device, dtype=torch.float32)
     tb, ts, nt = (0, 0, 0) if text is None else (text.stride(0), text.stride(1), text.shape[1])
     _call("other", _lib.lib().b2a_embed_sum, 1, codes.data_ptr(), codes.stride(0), B, G, tabs.dim, tabs.ptrs.data_ptr(), tabs.bins.data_ptr(),
-          _p(text), tb, ts, nt, _p(pad), _p(step_dev), step_sub, out.data_ptr(), out.stride(0), _p(err), _p(tidx), _p(finished), _stream())
+          _p(text), tb, ts, nt, _p(pad), out.data_ptr(), out.stride(0), _p(err), _p(tidx), _p(finished), _stream())
     return out
 
 

@@ -24,6 +24,7 @@ import torch
 
 from .... import ops
 from ...continuous import TTSBatchEvent, TTSBatchItem, TTSBatchOptions
+from .qwen3_tts import _capture_frame, _FrameState
 
 
 def _format_duration(seconds: float) -> str:
@@ -42,26 +43,6 @@ def _round_up(n: int, m: int) -> int:
 class _ActiveRequest:
     sequence_id: int
     slot: int
-
-
-class _FrameState:
-    """The buffers ``Model._frame`` reads and writes, for B rows.  ``_base_rows`` holds each row's cache length."""
-
-    def __init__(self, B: int, G: int, V: int, H: int, T: int, pad: torch.Tensor, suppress: torch.Tensor, dev):
-        self._kv_start, self._slot, self._prefill_len = None, None, 0
-        self._base_rows = torch.zeros(B, dtype=torch.int32, device=dev)
-        self._u = torch.zeros(G, B, device=dev)
-        self._suppress = suppress
-        self._seen = torch.zeros(B, V, dtype=torch.uint8, device=dev)
-        self._codes = torch.zeros(B, G, dtype=torch.int64, device=dev)
-        self._finished = torch.ones(B, dtype=torch.uint8, device=dev)              # empty slots are kept finished
-        self._cp_in0 = torch.zeros(B, 2, H, device=dev)
-        self._cp_in = torch.zeros(B, H, device=dev)
-        self._err = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._tidx = torch.zeros(B, dtype=torch.int32, device=dev)
-        self._pad = pad
-        self._trailing = pad.reshape(1, 1, H).expand(B, T, H).contiguous()         # pad-filled: rows past a request's text read pad
-        self._x_in = torch.zeros(B, 1, H, device=dev)
 
 
 class Qwen3TTSBatchSession:
@@ -86,7 +67,6 @@ class Qwen3TTSBatchSession:
         self.captures = 0                                   # CUDA graph captures of the frame (one per session unless a cache grows)
         self._graph = None
         self._use_graph = use_graph
-        self._frame_launches = 0
         self._sp = {"temperature": float(options.temperature), "top_k": int(options.top_k), "top_p": float(options.top_p),
                     "repetition_penalty": float(options.repetition_penalty), "eos": int(self.eos_token_id)}
         if options.max_tokens <= 0:
@@ -105,7 +85,9 @@ class Qwen3TTSBatchSession:
         cps = model.talker.code_predictor.stack
         shape = (len(cps.layers), n, _round_up(self._G + 1, 256), cps.n_kv * cps.hd)
         self._cp_kc, self._cp_vc = torch.zeros(shape, device=dev), torch.zeros(shape, device=dev)
-        self._st = _FrameState(n, self._G, self._V, self._H, 1, self._pad, self._suppress, dev)
+        self._st = _FrameState(n, self._G, self._pad_rows(n, 1), self._pad, self._suppress)
+        self._st._base_rows = torch.zeros(n, dtype=torch.int32, device=dev)
+        self._st._finished.fill_(1)                         # empty slots are kept finished
         self._frames = torch.zeros(n, dtype=torch.int32, device=dev)
         self._cap = torch.full((n,), int(options.max_tokens), dtype=torch.int32, device=dev)
         self._out = torch.zeros(n, int(options.max_tokens), self._G, dtype=torch.int64, device=dev)
@@ -165,30 +147,17 @@ class Qwen3TTSBatchSession:
             self._kc, self._vc, self._rows, self._graph = kc, vc, new, None
         if text_rows > self._T:
             new = _round_up(text_rows, 64)
-            tab = self._pad.reshape(1, 1, -1).expand(self._n, new, self._H).contiguous()
+            tab = self._pad_rows(self._n, new)
             tab[:, : self._st._trailing.shape[1]].copy_(self._st._trailing)
             self._st._trailing, self._T, self._graph = tab, new, None
+
+    def _pad_rows(self, B: int, T: int) -> torch.Tensor:
+        """A trailing-text table [B, T, H] filled with the pad embedding: rows past a request's text read pad."""
+        return self._pad.reshape(1, 1, -1).expand(B, T, self._H).contiguous()
 
     def _frame(self) -> None:
         self.model._frame(self._st._x_in, self._sp, self._st)
         ops.slot_advance(self._st._base_rows, self._frames, self._st._finished, self._cap, self._st._codes, self._out, self._utab, self._st._u)
-
-    def _capture(self) -> None:
-        """One eager frame (loads the S = 1 kernels) with the state restored afterwards, then the capture."""
-        st = self._st
-        bufs = [st._base_rows, self._frames, st._finished, st._seen, st._codes, st._x_in, st._tidx, st._u, st._err]
-        torch.cuda.synchronize(self._dev)
-        saved = [b.clone() for b in bufs]
-        l0 = ops.LAUNCHES[0]
-        self._frame()
-        self._frame_launches = ops.LAUNCHES[0] - l0
-        for b, s in zip(bufs, saved):
-            b.copy_(s)
-        torch.cuda.synchronize(self._dev)
-        self._graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self._graph):
-            self._frame()
-        self.captures += 1
 
     # ------------------------------------------------------------------ steps
     def _advance_active(self) -> list[TTSBatchEvent]:
@@ -197,7 +166,10 @@ class Qwen3TTSBatchSession:
                 self._frame()
             else:
                 if self._graph is None:
-                    self._capture()
+                    st = self._st
+                    self._graph, self._frame_launches = _capture_frame(self._frame, [st._base_rows, self._frames, st._finished, st._seen,
+                                                                                     st._codes, st._x_in, st._tidx, st._u, st._err])
+                    self.captures += 1
                 self._graph.replay()
                 ops.LAUNCHES[0] += self._frame_launches
         state = torch.cat([self._st._finished.int(), self._frames, self._st._err]).cpu()      # the step's one host read
@@ -230,8 +202,7 @@ class Qwen3TTSBatchSession:
         self._ensure_capacity(pmax + int(self.options.max_tokens) + 1, max(int(tr.shape[1]) for _, tr, _ in prep) + 1)
         # left-padded prompts [k, pmax, H]; row b's prompt lands at cache rows [0, P_b) of its slot
         x = torch.zeros(k, pmax, H, device=dev)
-        a = _FrameState(k, G, self._V, H, self._T, self._pad, self._suppress, dev)
-        a._finished.zero_()
+        a = _FrameState(k, G, self._pad_rows(k, self._T), self._pad, self._suppress)
         left = []
         for b, (e, tr, _) in enumerate(prep):
             left.append(pmax - int(e.shape[1]))

@@ -11,8 +11,9 @@ reference (per-row frame caps, joint decodes as one decoder batch), or to the ba
 
 One frame = talker step + first-codebook sample + 15 code-predictor sub-steps (each with its sampler) + next-input
 embedding sum: ~700 small launches.  They are captured ONCE into a CUDA graph; every scalar that changes between frames
-(KV length, trailing-text index, uniforms, seen-token set, codes) lives in device memory, so the host only replays the
-graph and reads back 16 integers per frame for the EOS test (the reference also syncs once per frame, :1398-1400).
+(KV length, trailing-text index, uniforms, seen-token set, codes, finished flags) lives in device memory, so the host only replays
+the graph and tests whether every row has finished every 8th frame (the reference syncs once per frame, :1398-1400).  A single
+sequence runs as a batch of one.
 """
 from __future__ import annotations
 
@@ -63,6 +64,47 @@ def mel_spectrogram(audio, n_fft: int = 1024, num_mels: int = 128, sample_rate: 
                            torch.as_tensor(basis, dtype=torch.float32).to(a.device).contiguous())
     window, basis = _MEL_CACHE[key]
     return ops.spk_logmel(a, window, basis)
+
+
+class _FrameState:
+    """The device buffers ``Model._frame`` reads and writes for B rows: ``trailing`` [B, n, H] text rows, ``pad`` [H], ``suppress`` [V].
+    How the talker addresses its cache is the one difference between callers: a static loop appends at the talker's device offset,
+    with ``_kv_start`` int32 [B] left-padding counts (None: none); a batch session sets ``_base_rows`` int32 [B] (each row's cache
+    length) and ``_slot`` (its cache slot)."""
+
+    def __init__(self, B: int, G: int, trailing: torch.Tensor, pad: torch.Tensor, suppress: torch.Tensor):
+        dev, H = pad.device, pad.numel()
+        self._kv_start = self._base_rows = self._slot = None
+        self._trailing, self._pad, self._suppress = trailing, pad, suppress
+        self._u = torch.zeros(G, B, device=dev)
+        self._seen = torch.zeros(B, suppress.numel(), dtype=torch.uint8, device=dev)
+        self._codes = torch.zeros(B, G, dtype=torch.int64, device=dev)
+        self._finished = torch.zeros(B, dtype=torch.uint8, device=dev)
+        self._tidx = torch.zeros(B, dtype=torch.int32, device=dev)
+        self._x_in = torch.zeros(B, 1, H, device=dev)
+        self._cp_in0 = torch.zeros(B, 2, H, device=dev)
+        self._cp_in = torch.zeros(B, H, device=dev)
+        self._err = torch.zeros(1, dtype=torch.int32, device=dev)
+
+
+def _capture_frame(frame, bufs):
+    """Capture ``frame()`` as a CUDA graph; returns (graph, launches per frame).  The frame first runs once eagerly, which loads the
+    S = 1 kernels and counts its launches, and ``bufs`` (the device buffers a frame advances) are restored before the capture.  Capture
+    records the kernels without running them, so the buffers still hold the pre-frame state afterwards; host-side mirrors (the
+    talker's ``offset``) are the caller's to reset."""
+    dev = bufs[0].device
+    torch.cuda.synchronize(dev)
+    saved = [b.clone() for b in bufs]
+    l0 = ops.LAUNCHES[0]
+    frame()
+    launches = ops.LAUNCHES[0] - l0
+    for b, s in zip(bufs, saved):
+        b.copy_(s)
+    torch.cuda.synchronize(dev)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        frame()
+    return graph, launches
 
 
 class Model:
@@ -297,19 +339,15 @@ class Model:
         return [i for i in range(cfg.vocab_size - 1024, cfg.vocab_size) if i != eos_token_id]
 
     # ------------------------------------------------------------------ frame loop
-    _base_rows = None       # per-row cache lengths and slot map of a batch session's frame state (continuous_batching.py); None here
-    _slot = None
-
-    def _frame(self, x_in: torch.Tensor, sp, st=None) -> None:
-        """One pass of the loop body qwen3_tts.py:1323-1398 for every batch row; results land in the state buffers of ``st`` (the
-        model's own for generate_codes, a batch session's otherwise -- its frames run at per-row cache lengths ``st._base_rows``)."""
-        st = self if st is None else st
+    def _frame(self, x_in: torch.Tensor, sp, st: _FrameState) -> None:
+        """One pass of the loop body qwen3_tts.py:1323-1398 for every row of ``st``, with the batch loop's rules (qwen3_tts.py:1880-1912):
+        a finished row samples EOS, and each row reads its own trailing-text row.  Results land in the buffers of ``st``."""
         t, cp = self.talker, self.talker.code_predictor
         g = self.config.talker_config.num_code_groups
-        if st._base_rows is not None:
-            logits, hidden = t(x_in, base_rows=st._base_rows, slot=st._slot)
-        else:
+        if st._base_rows is None:
             logits, hidden = t(x_in, use_device_offset=True, kv_start=st._kv_start)
+        else:
+            logits, hidden = t(x_in, base_rows=st._base_rows, slot=st._slot)
         ops.sample_token(logits[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=st._u[0],
                          suppress_mask=st._suppress, seen=st._seen, repetition_penalty=sp["repetition_penalty"], mark_seen=True,
                          out=st._codes[:, 0], finished=st._finished, eos=sp["eos"])
@@ -324,12 +362,9 @@ class Model:
                 lg = cp(e[:, None], ci + 1, ci)
             ops.sample_token(lg[:, -1], temperature=sp["temperature"], top_k=sp["top_k"], top_p=sp["top_p"], u=st._u[ci + 1],
                              out=st._codes[:, ci + 1])
-        if st._tidx is not None:        # batch rule: per-row trailing index, clamp-pad, advance unfinished rows (qwen3_tts.py:1903-1912)
-            ops.embed_sum(st._codes, self._tabs_all, text=st._trailing, pad=st._pad, out=st._x_in[:, 0], err=st._err,
-                          tidx=st._tidx, finished=st._finished)
-        else:
-            ops.embed_sum(st._codes, self._tabs_all, text=st._trailing, pad=st._pad, step_dev=t.offset_dev, step_sub=st._prefill_len,
-                          out=st._x_in[:, 0], err=st._err)
+        # per-row trailing index, clamp-pad, advance unfinished rows (qwen3_tts.py:1903-1912)
+        ops.embed_sum(st._codes, self._tabs_all, text=st._trailing, pad=st._pad, out=st._x_in[:, 0], err=st._err, tidx=st._tidx,
+                      finished=st._finished)
 
     def _uniform_stream(self, seed):
         """Generator the sampler's uniforms are drawn from.  ``seed=None`` continues ONE stream owned by the model, so successive
@@ -343,148 +378,108 @@ class Model:
         return self._rng
 
     @torch.no_grad()
-    def generate_codes(self, input_embeds, trailing_text_hidden, tts_pad_embed, **kw):
-        """The generation loop of Model.generate for B prompts of equal prefill length: returns int64 codes [B, n_frames, 16]
-        (B = 1: frames up to, not including, EOS; B > 1: until every row has hit EOS, rows padded with code 0 after their EOS,
-        the convention of batch_generate / batch_decode).  ``u`` [max_tokens, 16, B] uniforms in [0,1) (drawn from ``seed`` when
-        omitted; parity tests inject them).
+    def generate_codes(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, batch_mode: bool = False,
+                       trailing_rule: Optional[str] = None, **kw):
+        """The generation loop of Model.generate for B prompts (a single sequence is a batch of one): int64 codes [B, n, 16], each
+        row's frames up to (not including) its EOS or cap and code 0 after its end (the convention of batch_generate / batch_decode).
+        ``u`` [max_tokens, 16, B] uniforms in [0,1) (drawn from ``seed`` when omitted; parity tests inject them).
 
-        ``batch_mode`` = the loop of ``batch_generate`` (qwen3_tts.py:1861-1935): ``left_padding`` [B] rows of zero embeddings in front
-        of shorter prompts (masked keys, positions from cumsum(mask) - 1), ``trailing_text_hidden`` [B, n, H] right-padded with the
-        pad embedding, finished rows forced to EOS, per-row trailing indices with the clamp-pad rule; returns (codes [B, n, 16],
-        lengths [B]) with rows zero-padded after their EOS.  ``trailing_rule="standard"`` is the rule of the default (non-streaming)
+        ``batch_mode`` (implied by ``left_padding`` or ``caps``) returns (codes, lengths [B]) and defaults to the loop of
+        ``batch_generate``'s stream (qwen3_tts.py:1861-1935): ``left_padding`` [B] rows of zero embeddings in front of shorter prompts
+        (masked keys, positions from cumsum(mask) - 1), ``trailing_text_hidden`` [B, n, H] right-padded with the pad embedding, the
+        clamp-pad trailing rule.  ``trailing_rule="standard"``, the default otherwise, is the rule of Model.generate and of the default
         batch path, where every row behaves as a single sequence (continuous_batching.py:261-278: text while its index is inside the
-        trailing text, pad afterwards): one extra pad row is appended so that the kernel's clamp lands on it."""
-        frames = self._frame_iter(input_embeds, trailing_text_hidden, tts_pad_embed, **kw)
+        trailing text, pad afterwards)."""
+        batch_mode = batch_mode or kw.get("left_padding") is not None or kw.get("caps") is not None
+        frames = self._frame_iter(input_embeds, trailing_text_hidden, tts_pad_embed,
+                                  trailing_rule=trailing_rule or ("clamp_pad" if batch_mode else "standard"), **kw)
         while True:
             try:
                 next(frames)
             except StopIteration as stop:
-                return stop.value
+                codes, lengths = stop.value
+                return (codes, lengths) if batch_mode else codes
 
     @torch.no_grad()
     def _frame_iter(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, max_tokens: int = 4096, temperature: float = 0.9,
                     top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, u=None, seed: int = 0,
-                    use_graph: bool = True, stop_on_eos: bool = True, left_padding=None, batch_mode: bool = False,
-                    trailing_rule: str = "clamp_pad", caps=None, emit_every: Optional[int] = None):
-        """The loop of ``generate_codes`` as a generator: outside batch mode it yields (out, n) after every recorded frame -- ``out``
-        [B, max_tokens, 16] is the device buffer whose first n frames are final -- and returns what ``generate_codes`` returns.
-
-        Batch mode: ``caps`` [B] are per-row frame caps (the ICL rule of qwen3_tts.py:1818-1823, 1925-1932: a row that has recorded its
-        cap is finished, and forced to EOS from the next frame on); rows without caps get ``max_tokens``.  With ``emit_every`` = k the
-        loop yields (out, n, lengths [B] on the host) after every k-th frame -- rows advance in lockstep, so a row can only complete a
-        stream chunk there -- unless every row has finished, in which case the reference breaks before emitting (:1913-1932)."""
+                    use_graph: bool = True, left_padding=None, trailing_rule: str = "clamp_pad", caps=None,
+                    emit_every: Optional[int] = None):
+        """The loop of ``generate_codes`` as a generator that returns (codes [B, n, 16], lengths [B] on the host).  Finished rows are
+        forced to EOS and masked on the device; ``trailing_rule="standard"`` appends one pad row to the trailing text so that the
+        kernel's clamp lands on it.  ``caps`` [B] are per-row frame caps (the ICL rule of qwen3_tts.py:1818-1823, 1925-1932: a row that
+        has recorded its cap is finished, and forced to EOS from the next frame on); rows without caps get ``max_tokens``.  With
+        ``emit_every`` = k the loop yields (out, n, lengths [B] on the host) after every k-th frame -- ``out`` [B, max_tokens, 16] is
+        the device buffer whose first n frames are final; rows advance in lockstep, so a row can only complete a stream chunk there --
+        unless every row has finished, in which case the reference breaks before emitting (:1913-1932)."""
         t, cfg, dev = self.talker, self.config.talker_config, self.device
         x = input_embeds.to(dev).float().contiguous()
         B, P, H = x.shape
         g, V = cfg.num_code_groups, cfg.vocab_size
         eos = cfg.codec_eos_token_id
-        batch_mode = batch_mode or left_padding is not None
+        if trailing_rule not in ("clamp_pad", "standard"):
+            raise ValueError(f"trailing_rule must be 'clamp_pad' or 'standard', got {trailing_rule!r}")
         capped = caps is not None
         caps = [min(int(c), max_tokens) for c in caps] if capped else [max_tokens] * B
-        n_steps = max(caps) if batch_mode else max_tokens          # every row has finished by then: the cache needs no more rows
+        n_steps = max(caps)                                      # every row has finished by then: the cache needs no more rows
         if u is None:
             u = torch.rand(max_tokens, g, B, device=dev, generator=self._uniform_stream(seed))
         u = u.to(dev).float().contiguous()
         sp = {"temperature": float(temperature), "top_k": int(top_k), "top_p": float(top_p), "repetition_penalty": float(repetition_penalty),
               "eos": int(eos)}
-        self._kv_start = None
-        if left_padding is not None and any(int(v) for v in left_padding):
-            self._kv_start = torch.tensor([int(v) for v in left_padding], dtype=torch.int32, device=dev)
-        self._finished = torch.zeros(B, dtype=torch.uint8, device=dev) if batch_mode else None
-        self._tidx = torch.zeros(B, dtype=torch.int32, device=dev) if batch_mode else None
         t.reset_cache(B, P + n_steps + 1)
-        self._prefill_len = P
-        self._trailing = trailing_text_hidden.to(dev).float().expand(B, -1, -1).contiguous() if trailing_text_hidden.shape[0] != B \
-            else trailing_text_hidden.to(dev).float().contiguous()
-        self._pad = tts_pad_embed.to(dev).float().reshape(-1).contiguous()
-        if batch_mode and trailing_rule == "standard":
-            self._trailing = torch.cat([self._trailing, self._pad.reshape(1, 1, H).expand(B, 1, H)], dim=1).contiguous()
-        elif trailing_rule not in ("clamp_pad", "standard"):
-            raise ValueError(f"trailing_rule must be 'clamp_pad' or 'standard', got {trailing_rule!r}")
-        self._suppress = torch.zeros(V, device=dev)
-        self._suppress[torch.tensor(self._suppress_codec_tokens(eos), device=dev)] = float("-inf")
-        self._seen = torch.zeros(B, V, dtype=torch.uint8, device=dev)
-        self._codes = torch.zeros(B, g, dtype=torch.int64, device=dev)
-        self._u = torch.zeros(g, B, device=dev)
-        self._x_in = torch.zeros(B, 1, H, device=dev)
-        self._cp_in0 = torch.zeros(B, 2, H, device=dev)
-        self._cp_in = torch.zeros(B, H, device=dev)
-        self._err = torch.zeros(1, dtype=torch.int32, device=dev)
+        pad = tts_pad_embed.to(dev).float().reshape(-1).contiguous()
+        trailing = trailing_text_hidden.to(dev).float().expand(B, -1, -1)
+        if trailing_rule == "standard":
+            trailing = torch.cat([trailing, pad.reshape(1, 1, H).expand(B, 1, H)], dim=1)
+        suppress = torch.zeros(V, device=dev)
+        suppress[torch.tensor(self._suppress_codec_tokens(eos), device=dev)] = float("-inf")
+        st = _FrameState(B, g, trailing.contiguous(), pad, suppress)
+        if left_padding is not None and any(int(v) for v in left_padding):
+            st._kv_start = torch.tensor([int(v) for v in left_padding], dtype=torch.int32, device=dev)
         out = torch.zeros(B, max_tokens, g, dtype=torch.int64, device=dev)
-        lengths_dev = torch.zeros(B, dtype=torch.int64, device=dev)
+        lengths = torch.zeros(B, dtype=torch.int64, device=dev)
         caps_dev = torch.tensor(caps, dtype=torch.int64, device=dev)
         cap_hit = torch.zeros(B, dtype=torch.bool, device=dev)
-        done =torch.zeros(B, dtype=torch.bool)
+        frame = lambda: self._frame(st._x_in, sp, st)
         n = 0
         graph = None
         for step in range(n_steps):
-            self._u.copy_(u[step])
+            st._u.copy_(u[step])
             if step == 0:
-                self._frame(x, sp)                                                   # prefill frame (S = P rows), eager
-            elif use_graph:
+                self._frame(x, sp, st)                                               # prefill frame (S = P rows), eager
+            elif not use_graph:
+                frame()
+            else:
                 if graph is None:
                     # warm-up on a side stream is not needed: every kernel has already run once in the prefill frame except
-                    # the S = 1 GEMV variants, which the capture below launches for the first time (lazy module load is done).
-                    torch.cuda.synchronize(dev)
-                    bufs = [t.offset_dev, self._seen, self._codes, self._x_in] + ([self._finished, self._tidx] if batch_mode else [])
-                    state = [b_.clone() for b_ in bufs]
-                    restore = lambda: [b_.copy_(s_) for b_, s_ in zip(bufs, state)]
-                    l0 = ops.LAUNCHES[0]
-                    self._frame(self._x_in, sp)                                      # eager run of the S = 1 path (loads kernels)
-                    self._frame_launches = ops.LAUNCHES[0] - l0
-                    restore()
-                    t.offset = P + step - 1
-                    torch.cuda.synchronize(dev)
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        self._frame(self._x_in, sp)
-                    restore()
-                    t.offset = P + step - 1
+                    # the S = 1 GEMV variants, which the eager frame of the capture launches for the first time.
+                    graph, launches = _capture_frame(frame, [t.offset_dev, st._seen, st._codes, st._x_in, st._finished, st._tidx])
                 graph.replay()
-                t.offset = P + step
-                ops.LAUNCHES[0] += self._frame_launches
-            else:
-                l0 = ops.LAUNCHES[0]
-                self._frame(self._x_in, sp)
-                self._frame_launches = ops.LAUNCHES[0] - l0
-            if batch_mode:
-                # No per-frame host read: a finished row is masked on the device (its frame keeps the zeros `out` starts with, its length
-                # stops growing) and the all-finished test is a sync every 8th frame only -- the frames replayed past the last EOS record
-                # nothing.  (One .cpu() per frame held the loop at ~12 ms per frame; the graph itself replays in under 5.)
-                fin = self._finished.bool()
-                out[:, n] = torch.where(fin[:, None], out[:, n], self._codes)
-                lengths_dev += (~fin).to(torch.int64)
-                self._finished.bitwise_or_(torch.ge(lengths_dev, caps_dev, out=cap_hit))
-                n += 1
-                if emit_every and n % emit_every == 0:
-                    state = torch.cat([lengths_dev, self._finished.to(torch.int64)]).cpu()      # the one read per chunk boundary
-                    # without caps a row is never finished by max_tokens in the reference: the last frame still emits
-                    if bool(state[B:].all()) and (capped or n < n_steps):
-                        break
-                    yield out, n, state[:B]
-                elif (step & 7) == 7 and bool(self._finished.all()):
-                    break
-                continue
-            if stop_on_eos:
-                hit = self._codes[:, 0].cpu() == eos                                 # the per-frame sync (EOS test)
-                done |= hit
-                if bool(done.all()):
-                    break
-                live = ~done
-                out[live.to(dev), n] = self._codes[live.to(dev)]
-            else:
-                out[:, n] = self._codes
+                t.offset = P + step                                                  # the host mirror, which the capture advanced too
+                ops.LAUNCHES[0] += launches
+            # No per-frame host read: a finished row is masked on the device (its frame keeps the zeros `out` starts with, its length
+            # stops growing) and the all-finished test is a sync every 8th frame only -- the frames replayed past the last EOS record
+            # nothing.  (One .cpu() per frame held the loop at ~12 ms per frame; the graph itself replays in under 5.)
+            fin = st._finished.bool()
+            out[:, n] = torch.where(fin[:, None], out[:, n], st._codes)
+            lengths += (~fin).to(torch.int64)
+            st._finished.bitwise_or_(torch.ge(lengths, caps_dev, out=cap_hit))
             n += 1
-            yield out, n
-        if int(self._err.item()) != 0:
+            if emit_every and n % emit_every == 0:
+                state = torch.cat([lengths, st._finished.to(torch.int64)]).cpu()          # the one read per chunk boundary
+                # without caps a row is never finished by max_tokens in the reference: the last frame still emits
+                if bool(state[B:].all()) and (capped or n < n_steps):
+                    break
+                yield out, n, state[:B]
+            elif (step & 7) == 7 and bool(st._finished.all()):
+                break
+        if int(st._err.item()) != 0:
             raise ValueError("generate_codes: a sampled code indexed outside its embedding table")
         self._graph = graph
-        if batch_mode:
-            lengths = lengths_dev.cpu()
-            n = int(lengths.max()) if lengths.numel() else 0
-            return out[:, :n], lengths
-        return out[:, :n]
+        lengths = lengths.cpu()
+        n = int(lengths.max()) if lengths.numel() else 0
+        return out[:, :n], lengths
 
     # ------------------------------------------------------------------ batch generation
     def supports_tts_batch(self, *, stream: bool = False, voice: Optional[str] = None, instruct: Optional[str] = None, ref_audio=None,
@@ -555,11 +550,11 @@ class Model:
         t0 = time.perf_counter()
         x, trailing, pad, left = self.prepare_batch_inputs_from_ids(ids_list, language_id, speaker_ids)
         gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed,
-                   u=u, left_padding=left, batch_mode=True)
+                   u=u, left_padding=left)
         if stream:
             yield from self._stream_batch(x, trailing, pad, gen, streaming_interval, t0)
             return
-        codes, lengths = self.generate_codes(x, trailing, pad, trailing_rule="standard", **gen)
+        codes, lengths = self.generate_codes(x, trailing, pad, batch_mode=True, trailing_rule="standard", **gen)
         seqs = [codes[b, : int(lengths[b])] for b in range(codes.shape[0])]
         # rows of equal length share their decode launches: the chunks of _decode_generated_codes do not interact, so chunk j of every
         # row goes through the vocoder as one batch (identical samples; 8 rows x 3 chunks: 24 decoder passes -> 2)
@@ -721,11 +716,11 @@ class Model:
         per = [self.prepare_icl_generation_inputs_from_ids(ids, ref_ids, ref_codes, language_id, speaker_embed) for ids in target_ids_list]
         x, trailing, pad, left = self._pad_batch(per)
         gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed,
-                   u=u, left_padding=left, batch_mode=True, caps=row_max_tokens if row_max_tokens is not None else [max_tokens] * len(per))
+                   u=u, left_padding=left, caps=row_max_tokens if row_max_tokens is not None else [max_tokens] * len(per))
         if stream:
             yield from self._stream_batch(x, trailing, pad, gen, streaming_interval, t0)
             return
-        codes, lengths = self.generate_codes(x, trailing, pad, **gen)
+        codes, lengths = self.generate_codes(x, trailing, pad, batch_mode=True, **gen)
         dt = time.perf_counter() - t0
         rows = [b for b in range(codes.shape[0]) if int(lengths[b]) > 0]
         audios = self._decode_icl_batch([codes[b, : int(lengths[b])] for b in rows], ref_codes)
@@ -781,8 +776,8 @@ class Model:
             per = [self._prepare_generation_inputs(t, language=lang_code, speaker=v, instruct=i) for t, v, i in zip(texts, voices, instructs)]
             x, trailing, pad, left = self._pad_batch(per)
             yield from self._stream_batch(x, trailing, pad, dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
-                                                                 repetition_penalty=repetition_penalty, seed=seed, left_padding=left,
-                                                                 batch_mode=True), streaming_interval, time.perf_counter())
+                                                                 repetition_penalty=repetition_penalty, seed=seed, left_padding=left),
+                                          streaming_interval, time.perf_counter())
             return
         from ...continuous import TTSBatchItem, TTSBatchOptions
         from ..base import BatchGenerationResult
@@ -827,9 +822,10 @@ class Model:
         return audio
 
     def _stream_segment(self, x, trailing, pad, segment_idx: int, streaming_interval: float, gen: dict):
-        """The streaming branch of the generation loop (qwen3_tts.py:1316-1521, 2264-2446): after every recorded frame, once
-        ``max(1, int(streaming_interval * 12.5))`` frames are undecoded, decode them with the incremental decoder and yield a chunk;
-        after EOS / ``max_tokens`` yield the rest (if any) as the final chunk.  Streamed audio is not trimmed to the valid length."""
+        """The streaming branch of the generation loop (qwen3_tts.py:1316-1521, 2264-2446): once ``max(1, int(streaming_interval * 12.5))``
+        frames are undecoded, decode them with the incremental decoder and yield a chunk; after EOS / ``max_tokens`` yield the rest (if
+        any) as the final chunk.  The host reads the frame count only at chunk boundaries (``_frame_iter(emit_every=...)``).  Streamed
+        audio is not trimmed to the valid length."""
         dec = self.speech_tokenizer.decoder
         chunk = max(1, int(streaming_interval * 12.5))
         dec.reset_streaming_state()
@@ -853,11 +849,18 @@ class Model:
             t0 = time.perf_counter()
             return res
 
-        decoded, out, n = 0, None, 0
-        for out, n in self._frame_iter(x, trailing, pad, **gen):
-            if n - decoded >= chunk:
+        decoded = 0
+        frames = self._frame_iter(x, trailing, pad, trailing_rule="standard", emit_every=chunk, **gen)
+        while True:
+            try:
+                out, n, lengths = next(frames)
+            except StopIteration as stop:
+                out, lengths = stop.value
+                break
+            if int(lengths[0]) == n:
                 yield event(out[:1, decoded:n], n - decoded, n, False)
                 decoded = n
+        n = int(lengths[0])
         if n > decoded:
             yield event(out[:1, decoded:n], n - decoded, n, True)
         dec.reset_streaming_state()

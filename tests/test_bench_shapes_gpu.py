@@ -79,7 +79,7 @@ def test_qwen3_full_model_25_frames(g):
     ids = g["qwen3_ids"].tolist()
     got = model.prepare_generation_inputs_from_ids(ids, language_id=2050, speaker_id=2100)
     u = torch.rand(25, 16, generator=torch.Generator().manual_seed(2))
-    codes = model.generate_codes(*got, max_tokens=25, u=u[:, :, None], stop_on_eos=False)
+    codes = model.generate_codes(*got, max_tokens=25, u=u[:, :, None])
     want = torch.as_tensor(g["qwen3_codes"])
     assert codes.shape[1] >= want.shape[0]
     assert torch.equal(codes[0, : want.shape[0]].cpu(), want), (codes[0, : want.shape[0]].cpu() != want).nonzero()[:5]
