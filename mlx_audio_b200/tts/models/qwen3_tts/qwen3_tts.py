@@ -24,7 +24,7 @@ from typing import Dict, List, Optional
 import torch
 
 from .... import ops
-from ..base import GenerationResult
+from ..base import BatchGenerationResult, GenerationResult
 from .config import ModelConfig
 from .speaker_encoder import Qwen3TTSSpeakerEncoder
 from .speech_tokenizer import Qwen3TTSSpeechTokenizer
@@ -391,27 +391,23 @@ class Model:
         batch path, where every row behaves as a single sequence (continuous_batching.py:261-278: text while its index is inside the
         trailing text, pad afterwards)."""
         batch_mode = batch_mode or kw.get("left_padding") is not None or kw.get("caps") is not None
-        frames = self._frame_iter(input_embeds, trailing_text_hidden, tts_pad_embed,
-                                  trailing_rule=trailing_rule or ("clamp_pad" if batch_mode else "standard"), **kw)
-        while True:
-            try:
-                next(frames)
-            except StopIteration as stop:
-                codes, lengths = stop.value
-                return (codes, lengths) if batch_mode else codes
+        codes, _, lengths, _ = next(self._frame_iter(input_embeds, trailing_text_hidden, tts_pad_embed,
+                                                     trailing_rule=trailing_rule or ("clamp_pad" if batch_mode else "standard"), **kw))
+        return (codes, lengths) if batch_mode else codes
 
     @torch.no_grad()
     def _frame_iter(self, input_embeds, trailing_text_hidden, tts_pad_embed, *, max_tokens: int = 4096, temperature: float = 0.9,
                     top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, u=None, seed: int = 0,
                     use_graph: bool = True, left_padding=None, trailing_rule: str = "clamp_pad", caps=None,
                     emit_every: Optional[int] = None):
-        """The loop of ``generate_codes`` as a generator that returns (codes [B, n, 16], lengths [B] on the host).  Finished rows are
+        """The loop of ``generate_codes`` as a generator of (out, n, lengths [B] on the host, done); its last item, and without
+        ``emit_every`` its only one, has ``done`` set and ``out`` = codes [B, n, 16] with n the longest row.  Finished rows are
         forced to EOS and masked on the device; ``trailing_rule="standard"`` appends one pad row to the trailing text so that the
         kernel's clamp lands on it.  ``caps`` [B] are per-row frame caps (the ICL rule of qwen3_tts.py:1818-1823, 1925-1932: a row that
         has recorded its cap is finished, and forced to EOS from the next frame on); rows without caps get ``max_tokens``.  With
-        ``emit_every`` = k the loop yields (out, n, lengths [B] on the host) after every k-th frame -- ``out`` [B, max_tokens, 16] is
-        the device buffer whose first n frames are final; rows advance in lockstep, so a row can only complete a stream chunk there --
-        unless every row has finished, in which case the reference breaks before emitting (:1913-1932)."""
+        ``emit_every`` = k the loop also yields after every k-th frame -- ``out`` [B, max_tokens, 16] is the device buffer whose first
+        n frames are final; rows advance in lockstep, so a row can only complete a stream chunk there -- unless every row has
+        finished, in which case the reference breaks before emitting (:1913-1932)."""
         t, cfg, dev = self.talker, self.config.talker_config, self.device
         x = input_embeds.to(dev).float().contiguous()
         B, P, H = x.shape
@@ -471,7 +467,7 @@ class Model:
                 # without caps a row is never finished by max_tokens in the reference: the last frame still emits
                 if bool(state[B:].all()) and (capped or n < n_steps):
                     break
-                yield out, n, state[:B]
+                yield out, n, state[:B], False
             elif (step & 7) == 7 and bool(st._finished.all()):
                 break
         if int(st._err.item()) != 0:
@@ -479,7 +475,7 @@ class Model:
         self._graph = graph
         lengths = lengths.cpu()
         n = int(lengths.max()) if lengths.numel() else 0
-        return out[:, :n], lengths
+        yield out[:, :n], n, lengths, True
 
     # ------------------------------------------------------------------ batch generation
     def supports_tts_batch(self, *, stream: bool = False, voice: Optional[str] = None, instruct: Optional[str] = None, ref_audio=None,
@@ -544,7 +540,6 @@ class Model:
         15-frame chunks with 5 frames of left context (qwen3_tts.py:1050-1083).  ``stream=True`` follows the streaming branch
         (qwen3_tts.py:1861-2029): finished rows forced to EOS, clamp-pad trailing rule, and a chunk per row every ``streaming_interval``
         seconds of frames, then each row's remainder as its final chunk (``_stream_batch``)."""
-        from ..base import BatchGenerationResult
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
@@ -573,10 +568,7 @@ class Model:
         for b, s_ in enumerate(seqs):
             if s_.shape[0] == 0:
                 continue
-            a = next(it)
-            yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=int(s_.shape[0]),
-                                        audio_duration=format_duration(a.shape[0] / self.sample_rate), processing_time_seconds=dt,
-                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+            yield self._batch_result(next(it), b, int(s_.shape[0]), dt)
 
     def _stream_batch(self, x, trailing, pad, gen: dict, streaming_interval: float, t0: float):
         """The streaming branch of the static batch loop (qwen3_tts.py:1943-2029): once a row has ``max(1, int(streaming_interval * 12.5))``
@@ -584,23 +576,16 @@ class Model:
         reference hard-codes the 25); after the loop every row with undecoded frames emits them as its final chunk.  The host reads the
         row lengths only at chunk boundaries (``_frame_iter(emit_every=...)``)."""
         chunk = max(1, int(streaming_interval * 12.5))
-        B = x.shape[0]
-        decoded = [0] * B
-        frames = self._frame_iter(x, trailing, pad, emit_every=chunk, **gen)
-        while True:
-            try:
-                out, n, lengths = next(frames)
-            except StopIteration as stop:
-                out, lengths = stop.value
-                break
-            yield from self._emit_batch_chunks(out, [b for b in range(B) if int(lengths[b]) == n], decoded, [n] * B, False, t0)
-        ends = [int(v) for v in lengths]
-        yield from self._emit_batch_chunks(out, [b for b in range(B) if ends[b] > decoded[b]], decoded, ends, True, t0)
+        decoded = [0] * x.shape[0]
+        for out, n, lengths, done in self._frame_iter(x, trailing, pad, emit_every=chunk, **gen):
+            # in the loop the rows still running (length n) emit; at the end every row with undecoded frames does
+            ends = [int(v) for v in lengths]
+            rows = [b for b, e in enumerate(ends) if e > decoded[b] and (done or e == n)]
+            yield from self._emit_batch_chunks(out, rows, decoded, ends, done, t0)
 
     def _emit_batch_chunks(self, out, rows, decoded, ends, final: bool, t0: float):
         """One stream step of ``_stream_batch``: frames [decoded[b], ends[b]) of every row b in ``rows``, in row order.  Rows with equal
         context and chunk lengths go through one ``chunked_decode`` call (at an in-loop step that is every emitting row)."""
-        from ..base import BatchGenerationResult
         up = self.speech_tokenizer.decode_upsample_rate
         groups: Dict[tuple, List[int]] = {}
         for b in rows:
@@ -615,12 +600,16 @@ class Model:
         for b in rows:
             new = ends[b] - decoded[b]
             decoded[b] = ends[b]
-            a = audio[b]
-            yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=new,
-                                        audio_duration=format_duration(a.shape[0] / self.sample_rate),
-                                        processing_time_seconds=time.perf_counter() - t0,
-                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9, is_streaming_chunk=True,
-                                        is_final_chunk=final)
+            yield self._batch_result(audio[b], b, new, time.perf_counter() - t0, is_streaming_chunk=True, is_final_chunk=final)
+
+    def _batch_result(self, audio, sequence_idx: int, token_count: int, seconds: float, metadata=None, **flags):
+        """The BatchGenerationResult of one row's audio; a session event's ``metadata`` overrides the duration, time and memory fields."""
+        m = metadata or {}
+        return BatchGenerationResult(audio=audio, sequence_idx=sequence_idx, samples=int(audio.shape[0]), sample_rate=self.sample_rate,
+                                     token_count=token_count,
+                                     audio_duration=m.get("audio_duration", format_duration(audio.shape[0] / self.sample_rate)),
+                                     processing_time_seconds=m.get("processing_time_seconds", seconds),
+                                     peak_memory_usage=m.get("peak_memory_usage", torch.cuda.max_memory_allocated(self.device) / 1e9), **flags)
 
     # ------------------------------------------------------------------ batch_generate: requests, routes, ICL
     @staticmethod
@@ -703,16 +692,10 @@ class Model:
         row b stops on EOS or after ``row_max_tokens[b]`` frames (default ``max_tokens``).  ``u`` [max_tokens, 16, B] injects the uniforms.
         Yields one BatchGenerationResult per row with frames: [ref | generated] decoded together (one decoder batch for all rows), trimmed
         to the valid length, the reference's share cut off; or with ``stream=True`` chunks of the generated codes (``_stream_batch``)."""
-        from ..base import BatchGenerationResult
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
-        if ref_codes is None:
-            if ref_audio is None:
-                raise ValueError("batch_generate_icl_from_ids: pass ref_audio or ref_codes")
-            ref_codes = self.encode_reference(ref_audio)
-        if speaker_embed is None and ref_audio is not None and self.speaker_encoder is not None:
-            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        ref_codes, speaker_embed = self._resolve_icl_reference("batch_generate_icl_from_ids", ref_audio, ref_codes, speaker_embed)
         per = [self.prepare_icl_generation_inputs_from_ids(ids, ref_ids, ref_codes, language_id, speaker_embed) for ids in target_ids_list]
         x, trailing, pad, left = self._pad_batch(per)
         gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed,
@@ -725,9 +708,18 @@ class Model:
         rows = [b for b in range(codes.shape[0]) if int(lengths[b]) > 0]
         audios = self._decode_icl_batch([codes[b, : int(lengths[b])] for b in rows], ref_codes)
         for b, a in zip(rows, audios):
-            yield BatchGenerationResult(audio=a, sequence_idx=b, samples=int(a.shape[0]), sample_rate=self.sample_rate, token_count=int(lengths[b]),
-                                        audio_duration=format_duration(a.shape[0] / self.sample_rate), processing_time_seconds=dt,
-                                        peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+            yield self._batch_result(a, b, int(lengths[b]), dt)
+
+    def _resolve_icl_reference(self, caller: str, ref_audio, ref_codes, speaker_embed):
+        """(ref_codes, speaker_embed) of an in-context call: the reference's codes are encoded from ``ref_audio`` unless given, and its
+        x-vector takes the speaker row unless ``speaker_embed`` pins one (models with a speaker encoder)."""
+        if ref_codes is None:
+            if ref_audio is None:
+                raise ValueError(f"{caller}: pass ref_audio or ref_codes")
+            ref_codes = self.encode_reference(ref_audio)
+        if speaker_embed is None and ref_audio is not None and self.speaker_encoder is not None:
+            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        return ref_codes, speaker_embed
 
     def _icl_reference(self, ref_audio, ref_text):
         """(ref codes [1, 16, T], transcript ids) of a reference, cached on (ref_text, (size, sum) of ref_audio) (qwen3_tts.py:639-664)."""
@@ -780,7 +772,6 @@ class Model:
                                           streaming_interval, time.perf_counter())
             return
         from ...continuous import TTSBatchItem, TTSBatchOptions
-        from ..base import BatchGenerationResult
         session = self.create_tts_batch_session(TTSBatchOptions(temperature=temperature, top_p=top_p, top_k=top_k, repetition_penalty=repetition_penalty,
                                                                 max_tokens=max_tokens, lang_code=lang_code, stream=False,
                                                                 streaming_interval=streaming_interval, max_batch_size=B, verbose=verbose))
@@ -792,13 +783,8 @@ class Model:
                     raise ev.error
                 if ev.audio is None or ev.samples <= 0:
                     continue
-                yield BatchGenerationResult(audio=ev.audio, sequence_idx=ev.sequence_id, samples=ev.samples, sample_rate=ev.sample_rate,
-                                            token_count=ev.token_count,
-                                            audio_duration=ev.metadata.get("audio_duration", format_duration(ev.samples / self.sample_rate)),
-                                            processing_time_seconds=ev.metadata.get("processing_time_seconds", time.perf_counter() - t0),
-                                            peak_memory_usage=ev.metadata.get("peak_memory_usage",
-                                                                              torch.cuda.max_memory_allocated(self.device) / 1e9),
-                                            is_streaming_chunk=ev.is_streaming_chunk, is_final_chunk=ev.is_final_chunk)
+                yield self._batch_result(ev.audio, ev.sequence_id, ev.token_count, time.perf_counter() - t0, ev.metadata,
+                                         is_streaming_chunk=ev.is_streaming_chunk, is_final_chunk=ev.is_final_chunk)
 
     # ------------------------------------------------------------------ decode + public generate
     @torch.no_grad()
@@ -821,49 +807,51 @@ class Model:
             audio = audio[:valid]
         return audio
 
+    def _generation_result(self, audio, token_count: int, segment_idx: int, t0: float, is_streaming_chunk: bool = False,
+                           is_final_chunk: bool = False, total_tokens: Optional[int] = None) -> GenerationResult:
+        """The GenerationResult of ``audio`` decoded from ``token_count`` frames, timed from ``t0`` to the end of the work queued on the
+        device; a stream chunk before the last also reports ``total_tokens``, the frames generated so far (qwen3_tts.py:1440-1571)."""
+        torch.cuda.synchronize(self.device)
+        dt = time.perf_counter() - t0
+        samples = int(audio.shape[0])
+        dur = samples / self.sample_rate
+        audio_samples = {"samples": samples, "samples-per-sec": samples / dt if dt > 0 else 0}
+        if total_tokens is not None:
+            audio_samples["tokens"] = total_tokens
+        return GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=segment_idx, token_count=token_count,
+                                audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0,
+                                prompt={"tokens": token_count, "tokens-per-sec": token_count / dt if dt > 0 else 0}, audio_samples=audio_samples,
+                                processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9,
+                                is_streaming_chunk=is_streaming_chunk, is_final_chunk=is_final_chunk)
+
     def _stream_segment(self, x, trailing, pad, segment_idx: int, streaming_interval: float, gen: dict):
         """The streaming branch of the generation loop (qwen3_tts.py:1316-1521, 2264-2446): once ``max(1, int(streaming_interval * 12.5))``
         frames are undecoded, decode them with the incremental decoder and yield a chunk; after EOS / ``max_tokens`` yield the rest (if
         any) as the final chunk.  The host reads the frame count only at chunk boundaries (``_frame_iter(emit_every=...)``).  Streamed
-        audio is not trimmed to the valid length."""
+        audio is not trimmed to the valid length; each chunk is timed from the previous one."""
         dec = self.speech_tokenizer.decoder
         chunk = max(1, int(streaming_interval * 12.5))
         dec.reset_streaming_state()
-        t0 = time.perf_counter()
-
-        def event(codes, n_new, n_total, final):
-            nonlocal t0
-            audio = dec.streaming_step(codes.transpose(1, 2))[0, 0]
-            torch.cuda.synchronize(self.device)
-            dt = time.perf_counter() - t0
-            samples = int(audio.shape[0])
-            dur = samples / self.sample_rate
-            audio_samples = {"samples": samples, "samples-per-sec": samples / dt if dt > 0 else 0}
-            if not final:
-                audio_samples["tokens"] = n_total
-            res = GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=segment_idx, token_count=n_new,
-                                   audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0,
-                                   prompt={"tokens": n_new, "tokens-per-sec": n_new / dt if dt > 0 else 0}, audio_samples=audio_samples,
-                                   processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9,
-                                   is_streaming_chunk=True, is_final_chunk=final)
-            t0 = time.perf_counter()
-            return res
-
-        decoded = 0
-        frames = self._frame_iter(x, trailing, pad, trailing_rule="standard", emit_every=chunk, **gen)
-        while True:
-            try:
-                out, n, lengths = next(frames)
-            except StopIteration as stop:
-                out, lengths = stop.value
-                break
-            if int(lengths[0]) == n:
-                yield event(out[:1, decoded:n], n - decoded, n, False)
-                decoded = n
-        n = int(lengths[0])
-        if n > decoded:
-            yield event(out[:1, decoded:n], n - decoded, n, True)
+        t0, decoded = time.perf_counter(), 0
+        for out, n, lengths, done in self._frame_iter(x, trailing, pad, trailing_rule="standard", emit_every=chunk, **gen):
+            end = int(lengths[0])
+            if end > decoded and (done or end == n):             # in the loop only while the sequence is still running
+                audio = dec.streaming_step(out[:1, decoded:end].transpose(1, 2))[0, 0]
+                res = self._generation_result(audio, end - decoded, segment_idx, t0, is_streaming_chunk=True, is_final_chunk=done,
+                                              total_tokens=None if done else end)
+                t0, decoded = time.perf_counter(), end
+                yield res
         dec.reset_streaming_state()
+
+    def _run_segment(self, x, trailing, pad, segment_idx: int, t0: float, stream: bool, streaming_interval: float, gen: dict, decode):
+        """One segment from its prepared inputs: streamed by ``_stream_segment``, or generated in full, decoded by ``decode`` (codes
+        [1, n, 16] -> audio) and yielded as one GenerationResult timed from ``t0`` -- nothing when no frame was generated."""
+        if stream:
+            yield from self._stream_segment(x, trailing, pad, segment_idx, streaming_interval, gen)
+            return
+        codes = self.generate_codes(x, trailing, pad, **gen)
+        if codes.shape[1] > 0:
+            yield self._generation_result(decode(codes), int(codes.shape[1]), segment_idx, t0)
 
     def generate_from_ids(self, input_ids, *, language_id=None, speaker_id=None, temperature: float = 0.9, max_tokens: int = 4096,
                           top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.05, seed: int = 0, u=None,
@@ -879,24 +867,8 @@ class Model:
                 raise ValueError("Speaker encoder not available for this model type")
             speaker_embed = self.extract_speaker_embedding(ref_audio)
         x, trailing, pad = self.prepare_generation_inputs_from_ids(input_ids, language_id, speaker_id, speaker_embed=speaker_embed)
-        if stream:
-            yield from self._stream_segment(x, trailing, pad, 0, streaming_interval, dict(
-                max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u))
-            return
-        codes = self.generate_codes(x, trailing, pad, max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
-                                    repetition_penalty=repetition_penalty, seed=seed, u=u)
-        if codes.shape[1] == 0:
-            return
-        audio = self._decode_chunk(codes[:1])
-        torch.cuda.synchronize(self.device)
-        dt = time.perf_counter() - t0
-        samples = int(audio.shape[0])
-        dur = samples / self.sample_rate
-        yield GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=0, token_count=int(codes.shape[1]),
-                               audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0.0,
-                               prompt={"tokens": int(codes.shape[1]), "tokens-per-sec": round(codes.shape[1] / dt, 2) if dt > 0 else 0},
-                               audio_samples={"samples": samples, "samples-per-sec": round(samples / dt, 2) if dt > 0 else 0},
-                               processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+        gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u)
+        yield from self._run_segment(x, trailing, pad, 0, t0, stream, streaming_interval, gen, self._decode_chunk)
 
     def generate_icl_from_ids(self, target_ids, ref_ids, *, ref_audio=None, ref_codes=None, speaker_embed=None, language_id=None,
                               temperature: float = 0.9, max_tokens: int = 4096, top_k: int = 50, top_p: float = 1.0,
@@ -910,42 +882,18 @@ class Model:
         if self.speech_tokenizer is None:
             raise ValueError("Speech tokenizer not loaded")
         t0 = time.perf_counter()
-        if ref_codes is None:
-            if ref_audio is None:
-                raise ValueError("generate_icl_from_ids: pass ref_audio or ref_codes")
-            ref_codes = self.encode_reference(ref_audio)
-        if speaker_embed is None and ref_audio is not None and self.speaker_encoder is not None:
-            speaker_embed = self.extract_speaker_embedding(ref_audio)
+        ref_codes, speaker_embed = self._resolve_icl_reference("generate_icl_from_ids", ref_audio, ref_codes, speaker_embed)
         x, trailing, pad = self.prepare_icl_generation_inputs_from_ids(target_ids, ref_ids, ref_codes, language_id, speaker_embed)
         gen = dict(max_tokens=max_tokens, temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty, seed=seed, u=u)
-        if stream:
-            yield from self._stream_segment(x, trailing, pad, 0, streaming_interval, gen)
-            return
-        codes = self.generate_codes(x, trailing, pad, **gen)
-        if codes.shape[1] == 0:
-            return
-        audio = self._decode_icl_generated_codes(codes[0], ref_codes)
-        torch.cuda.synchronize(self.device)
-        dt = time.perf_counter() - t0
-        samples, n = int(audio.shape[0]), int(codes.shape[1])
-        dur = samples / self.sample_rate
-        yield GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=0, token_count=n,
-                               audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0.0,
-                               prompt={"tokens": n, "tokens-per-sec": n / dt if dt > 0 else 0},
-                               audio_samples={"samples": samples, "samples-per-sec": samples / dt if dt > 0 else 0},
-                               processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
-
-    @torch.no_grad()
-    def _decode_icl_generated_codes(self, gen_codes: torch.Tensor, ref_codes: torch.Tensor) -> torch.Tensor:
-        """qwen3_tts.py:1085-1112: gen_codes [n, 16] -> the target's audio: [ref | generated] decoded together, trimmed to the valid length
-        (frames whose first code is > 0), then int(T_ref / total * samples) samples of reference cut off the front."""
-        return self._decode_icl_batch([gen_codes], ref_codes)[0]
+        yield from self._run_segment(x, trailing, pad, 0, t0, stream, streaming_interval, gen,
+                                     lambda codes: self._decode_icl_batch([codes[0]], ref_codes)[0])
 
     @torch.no_grad()
     def _decode_icl_batch(self, gen_list, ref_codes) -> List[torch.Tensor]:
-        """``_decode_icl_generated_codes`` for several rows [n_b, 16] of one reference: the rows [ref | gen_b] go through the decoder as one
-        batch, right-padded with code 0.  Chunk boundaries count from frame 0 and the decoder is causal, so padding after a row's end does
-        not reach its frames; the valid lengths and cuts are each row's own."""
+        """qwen3_tts.py:1085-1112 for several rows [n_b, 16] of one reference: each row's audio is [ref | gen_b] decoded together, trimmed
+        to the valid length (frames whose first code is > 0), then int(T_ref / total * samples) samples of reference cut off the front.
+        The rows go through the decoder as one batch, right-padded with code 0.  Chunk boundaries count from frame 0 and the decoder is
+        causal, so padding after a row's end does not reach its frames; the valid lengths and cuts are each row's own."""
         up = self.speech_tokenizer.decode_upsample_rate
         ref_t = torch.as_tensor(ref_codes, dtype=torch.int64).to(self.device)[0].transpose(0, 1)
         totals = [ref_t.shape[0] + int(c.shape[0]) for c in gen_list]
@@ -985,22 +933,7 @@ class Model:
             seg_gen = dict(gen)
             if seg_gen.get("seed") is not None:                       # a fixed seed still gives every segment its own draws
                 seg_gen["seed"] = int(seg_gen["seed"]) + idx
-            if stream:                                                # the instruct paths report segment 0 (qwen3_tts.py:2264-2446)
-                yield from self._stream_segment(x, trailing, pad, idx if split_pattern else 0, streaming_interval, seg_gen)
-                continue
-            codes = self.generate_codes(x, trailing, pad, **seg_gen)
-            if codes.shape[1] == 0:
-                continue
-            audio = self._decode_chunk(codes[:1])
-            torch.cuda.synchronize(self.device)
-            dt = time.perf_counter() - t0
-            samples = int(audio.shape[0])
-            dur = samples / self.sample_rate
-            yield GenerationResult(audio=audio, samples=samples, sample_rate=self.sample_rate, segment_idx=idx, token_count=int(codes.shape[1]),
-                                   audio_duration=format_duration(dur), real_time_factor=dur / dt if dt > 0 else 0.0,
-                                   prompt={"tokens": int(codes.shape[1]), "tokens-per-sec": round(codes.shape[1] / dt, 2) if dt > 0 else 0},
-                                   audio_samples={"samples": samples, "samples-per-sec": round(samples / dt, 2) if dt > 0 else 0},
-                                   processing_time_seconds=dt, peak_memory_usage=torch.cuda.max_memory_allocated(self.device) / 1e9)
+            yield from self._run_segment(x, trailing, pad, idx, t0, stream, streaming_interval, seg_gen, self._decode_chunk)
 
     def generate(self, text: str, voice: Optional[str] = None, instruct: Optional[str] = None, temperature: float = 0.9, speed: float = 1.0,
                  lang_code: str = "auto", ref_audio=None, ref_text: Optional[str] = None, split_pattern: str = "\n", max_tokens: int = 4096,
