@@ -20,7 +20,7 @@ import torch
 
 from ... import ops
 from ...ops import ACT
-from .snac import _fold_wn
+from .descript_layers import wnconv
 
 
 @dataclass
@@ -151,9 +151,6 @@ class BigVGAN:
         f = lambda t: t.float().to(dev).contiguous()
         kaiser = kaiser_sinc_filter1d(0.25, 0.3, 12)                       # UpSample1d / DownSample1d at ratio 2 (resample.py:117-119, :146-151)
 
-        def wnconv(pre, except_dim=0):
-            return ops.pack_conv(_fold_wn(P[pre + ".weight_v"], P[pre + ".weight_g"], except_dim), P.get(pre + ".bias"), 1, dev)
-
         def act(pre):
             alpha, beta = P[pre + ".act.alpha"].double().reshape(-1), P[pre + ".act.beta"].double().reshape(-1)
             if cfg.snake_logscale:
@@ -161,19 +158,19 @@ class BigVGAN:
             fu, fd = P.get(pre + ".upsample.filter", kaiser), P.get(pre + ".downsample.lowpass.filter", kaiser)
             return f(alpha), f(1.0 / (beta + 1e-9)), f(fu.reshape(-1)), f(fd.reshape(-1))
 
-        W = {"pre": wnconv("conv_pre"), "stages": []}
+        W = {"pre": wnconv(P, "conv_pre", dev), "stages": []}
         for i, (u, k) in enumerate(zip(cfg.upsample_rates, cfg.upsample_kernel_sizes)):
             blocks = []
             for j, (kr, dil) in enumerate(zip(cfg.resblock_kernel_sizes, cfg.resblock_dilation_sizes)):
                 bp = f"resblocks.{i * self.num_kernels + j}"
                 if cfg.resblock == "1":
-                    units = [{"d": d, "c1": wnconv(f"{bp}.convs1.{m}"), "c2": wnconv(f"{bp}.convs2.{m}"),
+                    units = [{"d": d, "c1": wnconv(P, f"{bp}.convs1.{m}", dev), "c2": wnconv(P, f"{bp}.convs2.{m}", dev),
                               "a1": act(f"{bp}.activations.{2 * m}"), "a2": act(f"{bp}.activations.{2 * m + 1}")} for m, d in enumerate(dil)]
                 else:
-                    units = [{"d": d, "c1": wnconv(f"{bp}.convs.{m}"), "a1": act(f"{bp}.activations.{m}")} for m, d in enumerate(dil)]
+                    units = [{"d": d, "c1": wnconv(P, f"{bp}.convs.{m}", dev), "a1": act(f"{bp}.activations.{m}")} for m, d in enumerate(dil)]
                 blocks.append({"k": kr, "units": units})
-            W["stages"].append({"u": u, "k": k, "up": wnconv(f"ups.{i}.0", except_dim=2), "blocks": blocks})
-        W["post_act"], W["post"] = act("activation_post"), wnconv("conv_post")
+            W["stages"].append({"u": u, "k": k, "up": wnconv(P, f"ups.{i}.0", dev, except_dim=2), "blocks": blocks})
+        W["post_act"], W["post"] = act("activation_post"), wnconv(P, "conv_post", dev)
         self._W = W
         return self
 

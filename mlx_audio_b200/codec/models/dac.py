@@ -25,8 +25,8 @@ import numpy as np
 import torch
 
 from ... import ops
-from ...ops import ACT, Pre
-from .snac import _fold_wn
+from ...ops import ACT
+from .descript_layers import downsample, fold_wn, res_unit, res_units, snake, snapshot_dir, upsample, vq_level, wnconv
 
 SUPPORTED_VERSIONS = ["1.0.0"]
 
@@ -83,18 +83,12 @@ class ResidualVectorQuantize:
 
     def _load(self, P):
         dev = self.device
-        f = lambda t: t.float().to(dev).contiguous()
         self._levels, self._in_proj = [], []
         for i in range(self.n_codebooks):
-            q = f"quantizer.quantizers.{i}"
-            cb = P[q + ".codebook.weight"]
-            lv = {"cb": f(cb), "w_out": f(_fold_wn(P[q + ".out_proj.weight_v"], P[q + ".out_proj.weight_g"])[:, 0, :].t()),
-                  "b_out": f(P[q + ".out_proj.bias"])}
-            if q + ".in_proj.weight_v" in P:
-                cn = (cb.double() / cb.double().norm(dim=1, keepdim=True).clamp(min=1e-12)).float()   # the search runs on the normalised table
-                cw = ops.pack_conv(_fold_wn(P[q + ".in_proj.weight_v"], P[q + ".in_proj.weight_g"]), P[q + ".in_proj.bias"], 1, dev)
-                lv.update(cbn=f(cn), c2=(cn.double() ** 2).sum(1).to(dev).contiguous(), w_in=cw.w.reshape(self.input_dim, -1), b_in=cw.bias)
-                self._in_proj.append(cw)
+            lv = vq_level(P, f"quantizer.quantizers.{i}", dev)
+            if "in_proj" in lv:
+                lv.update(w_in=lv["in_proj"].w.reshape(self.input_dim, -1), b_in=lv["in_proj"].bias)
+                self._in_proj.append(lv["in_proj"])
             self._levels.append(lv)
         self._table = ops.dac_levels(self._levels, dev)
         self._cum = np.cumsum([0] + self.codebook_dim)
@@ -201,10 +195,7 @@ class DAC:
         """dac.py:251-272 for a LOCAL snapshot directory (config.json + model.safetensors); a hub id is resolved through
         huggingface_hub only when that package can reach it."""
         import json
-        path = Path(repo_id)
-        if not path.exists():
-            from huggingface_hub import snapshot_download
-            path = Path(snapshot_download(repo_id=repo_id, allow_patterns=["*.safetensors", "*.json"]))
+        path = snapshot_dir(repo_id)
         from safetensors.torch import load_file
         with open(path / "config.json") as f:
             config = json.load(f)
@@ -213,47 +204,28 @@ class DAC:
     def load_weights(self, weights, strict=True):
         P = dict(weights)
         dev = self.device
-        f = lambda t: t.float().to(dev).contiguous()
-
-        def wnconv(pre):
-            return ops.pack_conv(_fold_wn(P[pre + ".weight_v"], P[pre + ".weight_g"]), P.get(pre + ".bias"), 1, dev)
-
-        def snake(name):
-            a = P[name].float().reshape(-1)
-            return f(a), f(1.0 / (a + 1e-9))                                   # x + sin(a x)^2 / (a + 1e-9), nn/layers.py:116-119
-
-        def res_units(bp, first):
-            return [{"d": d, "s1": snake(f"{bp}.{first + i}.block.layers.0.alpha"), "c1": wnconv(f"{bp}.{first + i}.block.layers.1"),
-                     "s2": snake(f"{bp}.{first + i}.block.layers.2.alpha"), "c2": wnconv(f"{bp}.{first + i}.block.layers.3")}
-                    for i, d in enumerate((1, 3, 9))]
-
         self.quantizer._load(P)
         pre = "decoder.model.layers"
-        D = {"in": wnconv(f"{pre}.0"), "blocks": []}
+        D = {"in": wnconv(P, f"{pre}.0", dev), "blocks": []}
         for i, stride in enumerate(self.decoder_rates):
             bp = f"{pre}.{i + 1}.block.layers"
-            wt = _fold_wn(P[f"{bp}.1.weight_v"], P[f"{bp}.1.weight_g"], except_dim=2)       # (out, K, in): norm per INPUT channel, layers.py:91
-            D["blocks"].append({"stride": stride, "snake": snake(f"{bp}.0.alpha"), "up": ops.pack_conv(wt, P.get(f"{bp}.1.bias"), 1, dev),
-                                "res": res_units(bp, 2)})
+            wt = fold_wn(P[f"{bp}.1.weight_v"], P[f"{bp}.1.weight_g"], except_dim=2)        # (out, K, in): norm per INPUT channel, layers.py:91
+            D["blocks"].append({"stride": stride, "snake": snake(P, f"{bp}.0.alpha", dev), "up": ops.pack_conv(wt, P.get(f"{bp}.1.bias"), 1, dev),
+                                "res": res_units(P, bp, 2, 1, dev)})
         n = len(self.decoder_rates)
-        D["out_snake"], D["out"] = snake(f"{pre}.{n + 1}.alpha"), wnconv(f"{pre}.{n + 2}")
+        D["out_snake"], D["out"] = snake(P, f"{pre}.{n + 1}.alpha", dev), wnconv(P, f"{pre}.{n + 2}", dev)
         self._dec, self._enc = D, None
         if "encoder.block.layers.0.weight_v" in P:
             pre = "encoder.block.layers"
-            E = {"in": wnconv(f"{pre}.0"), "blocks": []}
+            E = {"in": wnconv(P, f"{pre}.0", dev), "blocks": []}
             for i, stride in enumerate(self.encoder_rates):
                 bp = f"{pre}.{i + 1}.block.layers"
-                E["blocks"].append({"stride": stride, "res": res_units(bp, 0), "snake": snake(f"{bp}.3.alpha"), "down": wnconv(f"{bp}.4")})
+                E["blocks"].append({"stride": stride, "res": res_units(P, bp, 0, 1, dev), "snake": snake(P, f"{bp}.3.alpha", dev),
+                                    "down": wnconv(P, f"{bp}.4", dev)})
             n = len(self.encoder_rates)
-            E["out_snake"], E["out"] = snake(f"{pre}.{n + 1}.alpha"), wnconv(f"{pre}.{n + 2}")
+            E["out_snake"], E["out"] = snake(P, f"{pre}.{n + 1}.alpha", dev), wnconv(P, f"{pre}.{n + 2}", dev)
             self._enc = E
         return self
-
-    @staticmethod
-    def _res_unit(y, ru):
-        """dac.py:16-33: Snake -> k7 dilated conv -> Snake -> 1x1 conv, plus the input."""
-        t = ops.conv1d(y, ru["c1"], dilation=ru["d"], pad_left=3 * ru["d"], pre=Pre(act=ACT["snake"], a=ru["s1"][0], b=ru["s1"][1]))
-        return ops.conv1d(t, ru["c2"], pre=Pre(act=ACT["snake"], a=ru["s2"][0], b=ru["s2"][1]), res=y)
 
     def preprocess(self, audio_data: torch.Tensor, sample_rate=None) -> torch.Tensor:
         """dac.py:182-191: right-pad [B, 1, n] to a multiple of the hop."""
@@ -273,11 +245,8 @@ class DAC:
         x = audio_data.to(device=self.device, dtype=torch.float32)
         y = ops.conv1d(x.reshape(x.shape[0], -1, 1).contiguous(), E["in"], pad_left=3)              # [B, 1, n] -> [B, n, 1]: same memory
         for blk in E["blocks"]:
-            for ru in blk["res"]:
-                y = self._res_unit(y, ru)
-            s = blk["stride"]
-            y = ops.conv1d(y, blk["down"], stride=s, pad_left=math.ceil(s / 2), pre=Pre(act=ACT["snake"], a=blk["snake"][0], b=blk["snake"][1]))
-        return ops.conv1d(y, E["out"], pad_left=1, pre=Pre(act=ACT["snake"], a=E["out_snake"][0], b=E["out_snake"][1]))
+            y = downsample(y, blk)
+        return ops.conv1d(y, E["out"], pad_left=1, pre=E["out_snake"])
 
     @torch.no_grad()
     def encode(self, audio_data: torch.Tensor, n_quantizers: Optional[int] = None):
@@ -292,13 +261,10 @@ class DAC:
         W = self._dec
         x = ops.conv1d(z_cl, W["in"], pad_left=3)
         for blk in W["blocks"]:
-            s, L, p = blk["stride"], x.shape[1], math.ceil(blk["stride"] / 2)
-            lout = (L - 1) * s - 2 * p + (2 * s - 1) + 1 + 1              # output_padding = 1 (the positional-argument quirk, module docstring)
-            y = ops.conv1d(x, blk["up"], stride=s, pad_left=p, lout=lout, pre=Pre(act=ACT["snake"], a=blk["snake"][0], b=blk["snake"][1]), transpose=True)
+            x = upsample(x, blk)
             for ru in blk["res"]:
-                y = self._res_unit(y, ru)
-            x = y
-        return ops.conv1d(x, W["out"], pad_left=3, pre=Pre(act=ACT["snake"], a=W["out_snake"][0], b=W["out_snake"][1]), post_act=ACT["tanh"])
+                x = res_unit(x, ru)
+        return ops.conv1d(x, W["out"], pad_left=3, pre=W["out_snake"], post_act=ACT["tanh"])
 
     def decode(self, z: torch.Tensor) -> torch.Tensor:
         """dac.py:204-205: z [B, D, T] -> audio [B, T_out, 1] -- channels-last, the reference does not move the axis back."""

@@ -13,19 +13,8 @@ from typing import List, Optional
 import torch
 
 from ... import ops
-from ...ops import ACT, Pre
-
-
-def _bf16(x):
-    return x.to(torch.bfloat16).to(torch.float32)
-
-
-def _fold_wn(v, g, except_dim=0):
-    """snac/layers.py:9-14,57: g * v / ||v||, folded once at load in the checkpoint's dtype (SNAC checkpoints are
-    float32 and the reference does not cast them, snac.py:184-199), so no rounding is applied."""
-    v, g = v.double(), g.double()
-    axes = tuple(i for i in range(v.dim()) if i != except_dim)
-    return (g * v / torch.sqrt((v * v).sum(dim=axes, keepdim=True))).float()
+from ...ops import ACT
+from .descript_layers import downsample, fold_wn, res_unit, res_units, snake, snapshot_dir, upsample, vq_level, wnconv
 
 
 class SNAC:
@@ -58,11 +47,7 @@ class SNAC:
     def from_pretrained(cls, repo_id, device="cuda", **kwargs):
         """snac.py:184-199 for a LOCAL snapshot directory (config.json + model.safetensors, already in the module-tree layout); a hub id
         is resolved through huggingface_hub only when that package can reach it."""
-        from pathlib import Path
-        path = Path(repo_id)
-        if not path.exists():
-            from huggingface_hub import snapshot_download
-            path = Path(snapshot_download(repo_id=repo_id, allow_patterns=["*.safetensors", "*.json"]))
+        path = snapshot_dir(repo_id)
         from safetensors.torch import load_file
         model = cls.from_config(path / "config.json", device=device)
         return model.load_weights(list(load_file(str(path / "model.safetensors")).items()))
@@ -74,68 +59,40 @@ class SNAC:
     def load_weights(self, weights, strict=True):
         P = dict(weights)
         dev = self.device
-        f = lambda t: t.float().to(dev).contiguous()
-
-        def wnconv(pre, groups=1):
-            return ops.pack_conv(_fold_wn(P[pre + ".weight_v"], P[pre + ".weight_g"]), P.get(pre + ".bias"), groups, dev)
-
-        def snake(name):
-            a = P[name].float().reshape(-1)
-            return f(a), f(1.0 / (a + 1e-9))                                   # x + sin(a x)^2 / (a + 1e-9), layers.py:124-130
-
-        W = {"emb": [], "proj_w": [], "proj_b": []}
-        for i in range(self.n_codebooks):
-            q = f"quantizer.quantizers.{i}"
-            W["emb"].append(f(P[q + ".codebook.weight"]))
-            w = _fold_wn(P[q + ".out_proj.weight_v"], P[q + ".out_proj.weight_g"])      # [D,1,cd]
-            W["proj_w"].append(f(w[:, 0, :].t()))                                          # [cd, D]
-            W["proj_b"].append(f(P[q + ".out_proj.bias"]))
+        W = {"q": [vq_level(P, f"quantizer.quantizers.{i}", dev) for i in range(self.n_codebooks)]}
+        W["from_codes"] = [[q[k] for q in W["q"]] for k in ("cb", "w_out", "b_out")]           # snac_from_codes' per-level tables
         pre = "decoder.model.layers"
         li = 0
         if self.depthwise:
-            W["in_dw"] = wnconv(f"{pre}.{li}", groups=self.latent_dim); li += 1
-            W["in_pw"] = wnconv(f"{pre}.{li}"); li += 1
+            W["in_dw"] = wnconv(P, f"{pre}.{li}", dev, groups=self.latent_dim); li += 1
+            W["in_pw"] = wnconv(P, f"{pre}.{li}", dev); li += 1
         else:
-            W["in_pw"] = wnconv(f"{pre}.{li}"); li += 1
+            W["in_pw"] = wnconv(P, f"{pre}.{li}", dev); li += 1
         W["blocks"] = []
         for i, stride in enumerate(self.decoder_rates):
             cout = self.decoder_dim // (2 ** (i + 1))
             bp = f"{pre}.{li}.block.layers"; li += 1
-            blk = {"stride": stride, "snake": snake(f"{bp}.0.alpha")}
-            wt = _fold_wn(P[f"{bp}.1.weight_v"], P[f"{bp}.1.weight_g"], except_dim=0).permute(2, 1, 0)     # (in,K,out)->(out,K,in)
+            blk = {"stride": stride, "snake": snake(P, f"{bp}.0.alpha", dev)}
+            wt = fold_wn(P[f"{bp}.1.weight_v"], P[f"{bp}.1.weight_g"], except_dim=0).permute(2, 1, 0)     # (in,K,out)->(out,K,in)
             blk["up"] = ops.pack_conv(wt, P.get(f"{bp}.1.bias"), 1, dev)
             bi = 2
             if self.noise:
-                blk["noise"] = wnconv(f"{bp}.{bi}.linear"); bi += 1
-            blk["res"] = []
-            for d in (1, 3, 9):
-                rp = f"{bp}.{bi}.block.layers"; bi += 1
-                blk["res"].append({"d": d, "s1": snake(rp + ".0.alpha"), "c1": wnconv(rp + ".1", groups=cout if self.depthwise else 1),
-                                   "s2": snake(rp + ".2.alpha"), "c2": wnconv(rp + ".3")})
+                blk["noise"] = wnconv(P, f"{bp}.{bi}.linear", dev); bi += 1
+            blk["res"] = res_units(P, bp, bi, cout if self.depthwise else 1, dev)
             W["blocks"].append(blk)
-        W["out_snake"] = snake(f"{pre}.{li}.alpha"); li += 1
-        W["out_conv"] = wnconv(f"{pre}.{li}")
+        W["out_snake"] = snake(P, f"{pre}.{li}.alpha", dev); li += 1
+        W["out_conv"] = wnconv(P, f"{pre}.{li}", dev)
         self._w = W
         self._enc = None
         if "encoder.block.layers.0.weight_v" in P:                     # encode side (snac/layers.py:133-158, vq.py:22-109)
-            E = {"in": wnconv("encoder.block.layers.0"), "blocks": [], "q": []}
+            E = {"in": wnconv(P, "encoder.block.layers.0", dev), "blocks": []}
             pre, li, d = "encoder.block.layers", 1, self.encoder_dim
             for stride in self.encoder_rates:
                 bp = f"{pre}.{li}.block.layers"; li += 1
-                blk = {"stride": stride, "res": [], "snake": snake(f"{bp}.3.alpha"), "down": wnconv(f"{bp}.4")}
-                for bi, dil in enumerate((1, 3, 9)):
-                    rp = f"{bp}.{bi}.block.layers"
-                    blk["res"].append({"d": dil, "s1": snake(rp + ".0.alpha"), "c1": wnconv(rp + ".1", groups=d if self.depthwise else 1),
-                                       "s2": snake(rp + ".2.alpha"), "c2": wnconv(rp + ".3")})
-                E["blocks"].append(blk)
+                E["blocks"].append({"stride": stride, "res": res_units(P, bp, 0, d if self.depthwise else 1, dev),
+                                    "snake": snake(P, f"{bp}.3.alpha", dev), "down": wnconv(P, f"{bp}.4", dev)})
                 d *= 2
-            E["out"] = wnconv(f"{pre}.{li}", groups=d if self.depthwise else 1)
-            for i in range(self.n_codebooks):
-                q = f"quantizer.quantizers.{i}"
-                cb = P[q + ".codebook.weight"].double()
-                cn = (cb / cb.norm(dim=1, keepdim=True).clamp(min=1e-12)).float()            # the cosine search runs on the L2-normalised table (vq.py:62-66)
-                E["q"].append({"in_proj": wnconv(q + ".in_proj"), "cn": f(cn)[None].contiguous(),
-                               "c2": (cn.double() ** 2).sum(1)[None].to(dev).contiguous()})
+            E["out"] = wnconv(P, f"{pre}.{li}", dev, groups=d if self.depthwise else 1)
             self._enc = E
         return self
 
@@ -145,35 +102,19 @@ class SNAC:
         ``noises[i]`` [B,1,C_i] injects the NoiseBlock draw (one per channel, layers.py:261-267); None draws it."""
         W, dev = self._w, self.device
         codes = [c.to(device=dev, dtype=torch.int64).contiguous() for c in codes]
-        z = ops.snac_from_codes(codes, self.vq_strides, W["emb"], W["proj_w"], W["proj_b"], self.latent_dim)     # [B,T,latent]
+        z = ops.snac_from_codes(codes, self.vq_strides, *W["from_codes"], self.latent_dim)                   # [B,T,latent]
         B = z.shape[0]
         x = ops.conv1d(z, W["in_dw"], pad_left=3) if self.depthwise else z
         x = ops.conv1d(x, W["in_pw"], pad_left=0 if self.depthwise else 3)
         for i, blk in enumerate(W["blocks"]):
-            s = blk["stride"]
-            L = x.shape[1]
-            p = math.ceil(s / 2)
-            lout = (L - 1) * s - 2 * p + (2 * s - 1) + 1 + 1          # output_padding = 1 (the reference's positional-arg quirk)
-            a, ia = blk["snake"]
-            y = ops.conv1d(x, blk["up"], stride=s, pad_left=p, lout=lout, pre=Pre(act=ACT["snake"], a=a, b=ia), transpose=True)
+            x = upsample(x, blk)
             if self.noise:
-                nz = noises[i] if noises is not None else torch.randn(B, 1, y.shape[2], device=dev)
+                nz = noises[i] if noises is not None else torch.randn(B, 1, x.shape[2], device=dev)
                 nz = nz.to(device=dev, dtype=torch.float32).reshape(B, -1).contiguous()
-                y = ops.conv1d(y, blk["noise"], cscale=nz, res=y)                   # x + noise * linear(x)
+                x = ops.conv1d(x, blk["noise"], cscale=nz, res=x)                   # x + noise * linear(x)
             for ru in blk["res"]:
-                s1 = Pre(act=ACT["snake"], a=ru["s1"][0], b=ru["s1"][1])
-                s2 = Pre(act=ACT["snake"], a=ru["s2"][0], b=ru["s2"][1])
-                if ru["c1"].groups > 1 and ru["c2"].w_tc is not None and ops.emit_eligible(ru["c1"], y, y.shape[1], dilation=ru["d"]) \
-                        and ru["c2"].cin_pad == ru["c1"].cout and ru["c2"].cin * ru["c2"].K >= ops.TC_MIN_K:
-                    # depthwise conv writes Snake2(t) as the 1x1 conv's bf16 planes: no fp32 t, no prologue pass
-                    t = ops.conv1d(y, ru["c1"], dilation=ru["d"], pad_left=3 * ru["d"], pre=s1, emit=s2)
-                    y = ops.conv1d(t, ru["c2"], res=y)
-                else:
-                    t = ops.conv1d(y, ru["c1"], dilation=ru["d"], pad_left=3 * ru["d"], pre=s1)
-                    y = ops.conv1d(t, ru["c2"], pre=s2, res=y)
-            x = y
-        a, ia = W["out_snake"]
-        return ops.conv1d(x, W["out_conv"], pad_left=3, pre=Pre(act=ACT["snake"], a=a, b=ia), post_act=ACT["tanh"])
+                x = res_unit(x, ru)
+        return ops.conv1d(x, W["out_conv"], pad_left=3, pre=W["out_snake"], post_act=ACT["tanh"])
 
     # halo (in finest-level frames) that makes a span decode EXACT: first conv +-3, per block the transposed conv (+-1) and three residual
     # units of kernel 7 with dilations 1 / 3 / 9 (+-39 samples at that block's rate: 39/8 + 39/64 + ... < 6 frames), last conv +-3/512.
@@ -233,20 +174,19 @@ class SNAC:
         level's stride, 1x1 projection to 8 dims, cosine nearest-code search (`rvq_encode_kernel`, first index on ties), project the code
         back, repeat by the stride, subtract from the residual (vq.py:22-109).  Needs a checkpoint that carries the encoder."""
         residual = self.encode_latent(audio_data)                                                              # [B, T, latent]
-        E = self._enc
         B, T, D = residual.shape
         codes = []
         for i, stride in enumerate(self.vq_strides):
-            q = E["q"][i]
+            q = self._w["q"][i]
             xl = residual
             if stride > 1:
                 t_ = (T - stride) // stride + 1
                 xl = (residual[:, : t_ * stride].reshape(B, t_, stride, D).sum(dim=2) / stride).contiguous()
             ze = ops.conv1d(xl, q["in_proj"])                                                                  # [B, T', cd]
-            idx = ops.rvq_encode(ze.reshape(-1, ze.shape[-1]), q["cn"], q["c2"], mode=1)[:, 0].reshape(B, -1).contiguous()
+            idx = ops.rvq_encode(ze.reshape(-1, ze.shape[-1]), q["cbn"][None], q["c2"][None], mode=1)[:, 0].reshape(B, -1).contiguous()
             codes.append(idx)
             if i + 1 < len(self.vq_strides):
-                zq = ops.snac_from_codes([idx], [stride], [self._w["emb"][i]], [self._w["proj_w"][i]], [self._w["proj_b"][i]], D, check=False)
+                zq = ops.snac_from_codes([idx], [stride], [q["cb"]], [q["w_out"]], [q["b_out"]], D, check=False)
                 residual = residual - zq[:, :T] if zq.shape[1] >= T else residual - torch.nn.functional.pad(zq, (0, 0, 0, T - zq.shape[1]))
         return codes
 
@@ -260,11 +200,5 @@ class SNAC:
         x = x.reshape(x.shape[0], -1, 1)                                                                       # [B, 1, n] -> [B, n, 1] (one channel: same memory)
         y = ops.conv1d(x, E["in"], pad_left=3)
         for blk in E["blocks"]:
-            for ru in blk["res"]:
-                s1 = Pre(act=ACT["snake"], a=ru["s1"][0], b=ru["s1"][1])
-                s2 = Pre(act=ACT["snake"], a=ru["s2"][0], b=ru["s2"][1])
-                t = ops.conv1d(y, ru["c1"], dilation=ru["d"], pad_left=3 * ru["d"], pre=s1)
-                y = ops.conv1d(t, ru["c2"], pre=s2, res=y)
-            s = blk["stride"]
-            y = ops.conv1d(y, blk["down"], stride=s, pad_left=math.ceil(s / 2), pre=Pre(act=ACT["snake"], a=blk["snake"][0], b=blk["snake"][1]))
+            y = downsample(y, blk)
         return ops.conv1d(y, E["out"], pad_left=3)
